@@ -336,6 +336,41 @@ typedef struct PxaDpmStepArgs {
 } PxaDpmStepArgs;
 int pxa_dpm_solver_pp_step(const PxaDpmStepArgs* args, void* stream);
 
+/* ------------------------------------------------------------------------------------ SA-Solver sampler step
+ * One fused elementwise pass per denoiser evaluation of the SA-Solver loop the reference runs in PyTorch as
+ * `SASolverSampler.sample` calls it (diffusion/sa_sampler.py:30-94: mode 'few_steps', skip_type 'time', predictor and
+ * corrector order 2, PEC, data prediction; call site scripts/inference.py:119-133).  Evaluation i (0 <= i < S) at time t_i:
+ *     eps      = eps_uncond + cfg_scale * (eps_cond - eps_uncond)    (guided; else the n conditional rows alone)
+ *     m        = (x_pred - sigma * eps) * inv_alpha                  (data prediction, diffusion/model/sa_solver.py:377-386)
+ *     x       <- c_x * x + c_m0 * m + c_m1 * m_prev + c_noise * noise_c      (corrector giving x_i, :700-753)
+ *     x_pred  <- p_x * x + p_m0 * m + p_m1 * m_prev + p_noise * noise_p      (predictor giving x~_{i+1}, :644-698)
+ *     m_prev  <- m
+ * (the predictor reads the corrected x).  The host computes every scalar once per evaluation: c_x = exp(-tau_i^2 h_i)
+ * sigma_i / sigma_{i-1}, c_noise = sigma_i sqrt(1 - exp(-2 tau_i^2 h_i)), c_m* the order-2 corrector gradient
+ * coefficients, and p_* the same for the step to t_{i+1} (order 1 at the first and the last step, tau = 0 at the last);
+ * i = 0 passes the identity corrector (c_x = 1, the others 0).  The loop driver: :841-897.
+ * `model_out` rows as in PxaDpmStepArgs (guided: [uncond (n) ; cond (n)]).  A term whose coefficient is 0 is not read, so
+ * m_prev may be uninitialised at i = 0 and noise_c / noise_p may be NULL when c_noise / p_noise is 0.
+ * fp32 arithmetic; x, x_pred, m_prev, noise_*: fp32 [n, 4, hw] contiguous.  HBM-bound: 48 (fp32 out) / 40 (bf16 out)
+ * algorithmic bytes per latent element with both noise terms.
+ */
+typedef struct PxaSaStepArgs {
+  const void* model_out;    /* [2n (guided) or n, >=4, hw], dtype out_dtype                          */
+  float* x;                 /* fp32 [n, 4, hw] in/out: x_{i-1} -> x_i                                */
+  float* x_pred;            /* fp32 [n, 4, hw] in/out: x~_i (the denoiser input) -> x~_{i+1}         */
+  float* m_prev;            /* fp32 [n, 4, hw] in/out: m_{i-1} -> m_i                                */
+  const float* noise_c;     /* fp32 [n, 4, hw] xi_i, or NULL when c_noise == 0                       */
+  const float* noise_p;     /* fp32 [n, 4, hw] xi_{i+1}, or NULL when p_noise == 0                   */
+  int64_t out_batch_stride; /* elements                                                              */
+  int32_t n, hw;
+  int32_t out_dtype;        /* PXA_DTYPE_*                                                           */
+  int32_t guided;           /* 1: CFG batch of 2n rows; 0: n conditional rows, cfg_scale ignored      */
+  float cfg_scale, sigma, inv_alpha;
+  float c_x, c_m0, c_m1, c_noise;
+  float p_x, p_m0, p_m1, p_noise;
+} PxaSaStepArgs;
+int pxa_sa_solver_step(const PxaSaStepArgs* args, void* stream);
+
 /* =============================================================================================== training backward
  * The reference trains through torch autograd (train_scripts/train.py:197 `accelerator.backward(loss)`, per-block
  * activation checkpointing diffusion/model/utils.py:28-45).  The entry points below are the backward twins of the forward

@@ -5,6 +5,8 @@ Only what the path `PixArtMS.forward -> 28 x PixArtMSBlock.forward` needs:
   lib.py     ctypes binding of libpixart_sm100.so
   model.py   host-side mirror of the reference model API (same names, ctor, state_dict layout)
   sampler.py DPM-Solver++ loop around the path (mirror of the reference's `diffusion.DPMS`), fused step kernel + CUDA graph
+  sa_sampler.py  SA-Solver loop (mirror of the reference's `diffusion.SASolverSampler`), fused predictor-corrector step
+             kernel + CUDA graph
   autograd.py / training.py  training path: the block's ops as autograd Functions over forward + backward kernels, IDDPM loss
   parallel.py  batch-sharded inference replicas; bucketed gradient all-reduce for data-parallel training
   vae.py / t5.py  the callers either side of the path on the same kernels: SDXL-VAE (diffusers' AutoencoderKL layout) and the
@@ -13,6 +15,7 @@ Only what the path `PixArtMS.forward -> 28 x PixArtMSBlock.forward` needs:
 """
 from .model import (MODELS, PixArt, PixArt_XL_2, PixArtBlock, PixArtMS, PixArtMS_XL_2, PixArtMSBlock,  # noqa: F401
                     build_model, install_into_reference, set_grad_checkpoint)
+from .sa_sampler import SASolverSampler  # noqa: F401
 from .sampler import DPMS, DPMSolverPP  # noqa: F401
 
 __version__ = "0.1.0"

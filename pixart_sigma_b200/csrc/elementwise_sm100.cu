@@ -218,6 +218,46 @@ extern "C" int pxa_kv_compress_conv2_ln(const PxaKvCompressArgs* args, void* str
 
 namespace pxa {
 
+// ------------------------------------------------------------------------------------------------- sampler steps
+// Shared by the DPM-Solver++ and SA-Solver steps: 4 consecutive elements of one denoiser output row (fp32 or bf16).
+template <typename OT>
+PXA_DEVICE void load4(const OT* __restrict__ p, float (&v)[4]) {
+  if constexpr (sizeof(OT) == 4) {
+    const float4 u = *reinterpret_cast<const float4*>(p);
+    v[0] = u.x; v[1] = u.y; v[2] = u.z; v[3] = u.w;
+  } else {
+    const uint2 u = *reinterpret_cast<const uint2*>(p);
+    v[0] = bf16_lo(u.x); v[1] = bf16_hi(u.x); v[2] = bf16_lo(u.y); v[3] = bf16_hi(u.y);
+  }
+}
+
+// CFG combine + data prediction of 4 elements at offset e of image img:
+//   eps = eps_u + cfg * (eps_c - eps_u)  (guided: rows [uncond (n) ; cond (n)]),  eps = eps_c  (unguided: n rows)
+//   x0  = (xs - sigma * eps) * inv_alpha
+// Channel ch of row r is at mo[r * obs + ch * hw + p], so the image's [4, hw] block is a contiguous prefix of its row.
+template <typename OT, bool kGuided>
+PXA_DEVICE void cfg_data_pred4(const OT* __restrict__ mo, long long obs, int n, int img, int e, float cfg, float sigma,
+                               float inv_alpha, const float (&xs)[4], float (&x0)[4]) {
+  float ec[4];
+  load4<OT>(mo + (size_t)(kGuided ? img + n : img) * obs + e, ec);
+  float eu[4] = {0.f, 0.f, 0.f, 0.f};
+  if constexpr (kGuided) load4<OT>(mo + (size_t)img * obs + e, eu);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float eps = kGuided ? eu[k] + cfg * (ec[k] - eu[k]) : ec[k];
+    x0[k] = (xs[k] - sigma * eps) * inv_alpha;
+  }
+}
+
+PXA_DEVICE void load4f(const float* __restrict__ p, float (&v)[4]) {
+  const float4 u = *reinterpret_cast<const float4*>(p);
+  v[0] = u.x; v[1] = u.y; v[2] = u.z; v[3] = u.w;
+}
+
+PXA_DEVICE void store4f(float* __restrict__ p, const float (&v)[4]) {
+  *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+}
+
 // ------------------------------------------------------------------------------------------------- DPM-Solver++ step
 // One thread per 4 consecutive latent elements (hw % 4 == 0): CFG combine + data prediction + multistep update.
 template <typename OT>
@@ -230,37 +270,92 @@ __global__ void __launch_bounds__(256) dpm_step_kernel(const OT* __restrict__ mo
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int img = (int)(i / per_img);
     const int e = (int)(i - (long long)img * per_img) * 4;   // element offset inside the image's [4, hw] block
-    const OT* pu = mo + (size_t)img * obs + e;               // channel ch at ch*hw + p == contiguous [4, hw] prefix
-    const OT* pc = mo + (size_t)(img + n) * obs + e;
-    float eu[4], ec[4];
-    if constexpr (sizeof(OT) == 4) {
-      const float4 u = *reinterpret_cast<const float4*>(pu), v = *reinterpret_cast<const float4*>(pc);
-      eu[0] = u.x; eu[1] = u.y; eu[2] = u.z; eu[3] = u.w;
-      ec[0] = v.x; ec[1] = v.y; ec[2] = v.z; ec[3] = v.w;
-    } else {
-      const uint2 u = *reinterpret_cast<const uint2*>(pu), v = *reinterpret_cast<const uint2*>(pc);
-      eu[0] = bf16_lo(u.x); eu[1] = bf16_hi(u.x); eu[2] = bf16_lo(u.y); eu[3] = bf16_hi(u.y);
-      ec[0] = bf16_lo(v.x); ec[1] = bf16_hi(v.x); ec[2] = bf16_lo(v.y); ec[3] = bf16_hi(v.y);
-    }
     const size_t off = (size_t)img * 4 * hw + e;
-    const float4 xv = *reinterpret_cast<const float4*>(x + off);
-    float4 pv = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (c != 0.f) pv = *reinterpret_cast<const float4*>(x0_prev + off);
-    const float xs[4] = {xv.x, xv.y, xv.z, xv.w};
-    const float ps[4] = {pv.x, pv.y, pv.z, pv.w};
-    float xn[4], x0[4];
+    float xs[4], ps[4] = {0.f, 0.f, 0.f, 0.f}, xn[4], x0[4];
+    load4f(x + off, xs);
+    if (c != 0.f) load4f(x0_prev + off, ps);
+    cfg_data_pred4<OT, true>(mo, obs, n, img, e, cfg, sigma_s, inv_alpha_s, xs, x0);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) xn[k] = a * xs[k] - b * x0[k] - c * (x0[k] - ps[k]);
+    store4f(x + off, xn);
+    store4f(x0_prev + off, x0);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------- SA-Solver step
+// One thread per 4 consecutive latent elements: CFG combine + data prediction of the evaluation at x_pred, then the
+// corrector (x) and the next predictor (x_pred) from the same m.  A term whose coefficient is 0 is not read.
+template <typename OT, bool kGuided>
+__global__ void __launch_bounds__(256) sa_step_kernel(const OT* __restrict__ mo, float* __restrict__ x,
+                                                      float* __restrict__ x_pred, float* __restrict__ m_prev,
+                                                      const float* __restrict__ noise_c, const float* __restrict__ noise_p,
+                                                      long long obs, int n, int hw, float cfg, float sigma,
+                                                      float inv_alpha, float c_x, float c_m0, float c_m1, float c_noise,
+                                                      float p_x, float p_m0, float p_m1, float p_noise) {
+  const int per_img = hw;
+  const long long total = (long long)n * per_img;
+  const bool need_prev = c_m1 != 0.f || p_m1 != 0.f;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int img = (int)(i / per_img);
+    const int e = (int)(i - (long long)img * per_img) * 4;
+    const size_t off = (size_t)img * 4 * hw + e;
+    float xp[4], xs[4], m[4], mp[4] = {0.f, 0.f, 0.f, 0.f}, nc[4] = {0.f, 0.f, 0.f, 0.f}, np_[4] = {0.f, 0.f, 0.f, 0.f};
+    load4f(x_pred + off, xp);
+    load4f(x + off, xs);
+    if (need_prev) load4f(m_prev + off, mp);
+    if (c_noise != 0.f) load4f(noise_c + off, nc);
+    if (p_noise != 0.f) load4f(noise_p + off, np_);
+    cfg_data_pred4<OT, kGuided>(mo, obs, n, img, e, cfg, sigma, inv_alpha, xp, m);
+    float xc[4], xn[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float eps = eu[k] + cfg * (ec[k] - eu[k]);
-      x0[k] = (xs[k] - sigma_s * eps) * inv_alpha_s;
-      xn[k] = a * xs[k] - b * x0[k] - c * (x0[k] - ps[k]);
+      xc[k] = c_x * xs[k] + (c_m0 * m[k] + c_m1 * mp[k]) + c_noise * nc[k];
+      xn[k] = p_x * xc[k] + (p_m0 * m[k] + p_m1 * mp[k]) + p_noise * np_[k];
     }
-    *reinterpret_cast<float4*>(x + off) = make_float4(xn[0], xn[1], xn[2], xn[3]);
-    *reinterpret_cast<float4*>(x0_prev + off) = make_float4(x0[0], x0[1], x0[2], x0[3]);
+    store4f(x + off, xc);
+    store4f(x_pred + off, xn);
+    store4f(m_prev + off, m);
   }
 }
 
 }  // namespace pxa
+
+extern "C" int pxa_sa_solver_step(const PxaSaStepArgs* args, void* stream) {
+  using namespace pxa;
+  if (!args) return fail(PXA_ERR_ARG, "null args");
+  const PxaSaStepArgs& a = *args;
+  if (!a.model_out || !a.x || !a.x_pred || !a.m_prev) return fail(PXA_ERR_ARG, "null pointer");
+  if ((a.c_noise != 0.f && !a.noise_c) || (a.p_noise != 0.f && !a.noise_p))
+    return fail(PXA_ERR_ARG, "noise_c / noise_p required when their coefficient is non-zero");
+  if (a.n <= 0 || a.hw <= 0 || (a.hw & 3)) return fail(PXA_ERR_ARG, "n > 0 and hw a positive multiple of 4 required (n=%d hw=%d)", a.n, a.hw);
+  if (a.out_batch_stride < 4LL * a.hw) return fail(PXA_ERR_ARG, "out_batch_stride smaller than 4*hw");
+  if (a.guided != 0 && a.guided != 1) return fail(PXA_ERR_ARG, "guided must be 0 or 1");
+  const int esz = a.out_dtype == PXA_DTYPE_F32 ? 4 : 2;
+  if (a.out_dtype != PXA_DTYPE_F32 && a.out_dtype != PXA_DTYPE_BF16) return fail(PXA_ERR_ARG, "out_dtype must be PXA_DTYPE_F32 or PXA_DTYPE_BF16");
+  if ((reinterpret_cast<uintptr_t>(a.model_out) & (4 * esz - 1)) || ((a.out_batch_stride * esz) & (4 * esz - 1)) ||
+      ((reinterpret_cast<uintptr_t>(a.x) | reinterpret_cast<uintptr_t>(a.x_pred) | reinterpret_cast<uintptr_t>(a.m_prev) |
+        reinterpret_cast<uintptr_t>(a.noise_c) | reinterpret_cast<uintptr_t>(a.noise_p)) & 15))
+    return fail(PXA_ERR_ALIGN, "model_out / x / x_pred / m_prev / noise must be aligned to 4 elements");
+  PXA_REQUIRE_SM90();
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const long long total = (long long)a.n * a.hw;
+  int grid = (int)((total + 255) / 256);
+  const int cap = device_info().sms * 8;
+  if (grid > cap) grid = cap;
+#define PXA_SA_LAUNCH(OT, G)                                                                                              \
+  sa_step_kernel<OT, G><<<grid, 256, 0, s>>>(reinterpret_cast<const OT*>(a.model_out), a.x, a.x_pred, a.m_prev, a.noise_c, \
+                                             a.noise_p, a.out_batch_stride, a.n, a.hw, a.cfg_scale, a.sigma, a.inv_alpha,  \
+                                             a.c_x, a.c_m0, a.c_m1, a.c_noise, a.p_x, a.p_m0, a.p_m1, a.p_noise)
+  if (a.out_dtype == PXA_DTYPE_F32) {
+    if (a.guided) PXA_SA_LAUNCH(float, true); else PXA_SA_LAUNCH(float, false);
+  } else {
+    if (a.guided) PXA_SA_LAUNCH(__nv_bfloat16, true); else PXA_SA_LAUNCH(__nv_bfloat16, false);
+  }
+#undef PXA_SA_LAUNCH
+  launch_counter()++;
+  PXA_CHECK_CUDA(cudaGetLastError());
+  return PXA_OK;
+}
 
 extern "C" int pxa_dpm_solver_pp_step(const PxaDpmStepArgs* args, void* stream) {
   using namespace pxa;

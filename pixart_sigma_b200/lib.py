@@ -104,6 +104,15 @@ class DpmStepArgs(C.Structure):
                 ("a", C.c_float), ("b", C.c_float), ("c", C.c_float)]
 
 
+class SaStepArgs(C.Structure):
+    _fields_ = [("model_out", C.c_void_p), ("x", C.c_void_p), ("x_pred", C.c_void_p), ("m_prev", C.c_void_p),
+                ("noise_c", C.c_void_p), ("noise_p", C.c_void_p), ("out_batch_stride", C.c_int64),
+                ("n", C.c_int32), ("hw", C.c_int32), ("out_dtype", C.c_int32), ("guided", C.c_int32),
+                ("cfg_scale", C.c_float), ("sigma", C.c_float), ("inv_alpha", C.c_float),
+                ("c_x", C.c_float), ("c_m0", C.c_float), ("c_m1", C.c_float), ("c_noise", C.c_float),
+                ("p_x", C.c_float), ("p_m0", C.c_float), ("p_m1", C.c_float), ("p_noise", C.c_float)]
+
+
 class GateResidualArgs(C.Structure):
     _fields_ = [("x", C.c_void_p), ("y", C.c_void_p), ("gate", C.c_void_p), ("out", C.c_void_p), ("dgate", C.c_void_p),
                 ("gate_batch_stride", C.c_int64), ("rows_per_batch", C.c_int32), ("M", C.c_int32), ("C", C.c_int32)]
@@ -140,7 +149,7 @@ EXPORTS = ("pxa_transpose_bf16", "pxa_gelu_tanh_bf16", "pxa_gate_residual_fwd", 
            "pxa_version", "pxa_last_error", "pxa_launch_count", "pxa_gemm_bf16", "pxa_ln_modulate",
            "pxa_flash_attn_d72_bf16", "pxa_kv_compress_conv2_ln", "pxa_conv3x3_nhwc_bf16", "pxa_dpm_solver_pp_step",
            "pxa_ln_prepare", "pxa_layernorm_affine_bf16", "pxa_groupnorm_silu_nhwc_bf16", "pxa_adamw_flat", "pxa_mlp_fused_bf16",
-           "pxa_rmsnorm_bf16", "pxa_t5_attn_d64_bf16")
+           "pxa_rmsnorm_bf16", "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step")
 
 _lib = None
 
@@ -159,7 +168,8 @@ def load() -> C.CDLL:
                              ("pxa_flash_attn_d72_bf16", AttnArgs), ("pxa_kv_compress_conv2_ln", KvCompressArgs),
                              ("pxa_conv3x3_nhwc_bf16", Conv3x3Args), ("pxa_dpm_solver_pp_step", DpmStepArgs),
                              ("pxa_ln_prepare", LnPrepareArgs), ("pxa_adamw_flat", AdamWArgs),
-                             ("pxa_mlp_fused_bf16", MlpArgs), ("pxa_t5_attn_d64_bf16", T5AttnArgs)):
+                             ("pxa_mlp_fused_bf16", MlpArgs), ("pxa_t5_attn_d64_bf16", T5AttnArgs),
+                             ("pxa_sa_solver_step", SaStepArgs)):
             fn = getattr(lib, name)
             fn.restype = C.c_int
             fn.argtypes = [C.POINTER(struct), C.c_void_p]
@@ -458,6 +468,31 @@ def dpm_solver_pp_step(model_out: torch.Tensor, x: torch.Tensor, x0_prev: torch.
                        inv_alpha_s=1.0 / alpha_s, a=a, b=b, c=c)
     _check(load().pxa_dpm_solver_pp_step(C.byref(args), _stream()), "pxa_dpm_solver_pp_step")
     return x
+
+
+def sa_solver_step(model_out: torch.Tensor, x: torch.Tensor, x_pred: torch.Tensor, m_prev: torch.Tensor,
+                   noise_c: Optional[torch.Tensor], noise_p: Optional[torch.Tensor], *, guided: bool, cfg_scale: float,
+                   sigma: float, alpha: float, c_x: float, c_m0: float, c_m1: float, c_noise: float, p_x: float,
+                   p_m0: float, p_m1: float, p_noise: float) -> torch.Tensor:
+    """One SA-Solver evaluation step (corrector to x_i, predictor to x~_{i+1}), in place on x, x_pred and m_prev
+    (include/pixart_sm100.h: pxa_sa_solver_step); returns x_pred.  model_out: denoiser output at x_pred, (2n, C>=4, h, w)
+    [uncond; cond] when guided else (n, C>=4, h, w), fp32 or bf16 -- a channel-sliced view of the 8-channel learn-sigma
+    output is fine; x, x_pred, m_prev and the noise tensors: fp32 (n, 4, h, w) contiguous.  A noise tensor may be None
+    when its coefficient is 0."""
+    state = [x, x_pred, m_prev] + [t for t in (noise_c, noise_p) if t is not None]
+    assert model_out.is_cuda and all(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() for t in state)
+    assert x.dim() == 4 and x.shape[1] == 4 and all(t.shape == x.shape for t in state)
+    assert (noise_c is not None or c_noise == 0.0) and (noise_p is not None or p_noise == 0.0)
+    n, _, h, w = x.shape
+    assert model_out.shape[0] == (2 * n if guided else n) and model_out.shape[1] >= 4 and model_out.shape[2:] == (h, w)
+    assert model_out.stride(3) == 1 and model_out.stride(2) == w and model_out.stride(1) == h * w, "model_out: (.., h, w) planes must be dense"
+    args = SaStepArgs(model_out=_ptr(model_out), x=_ptr(x), x_pred=_ptr(x_pred), m_prev=_ptr(m_prev), noise_c=_ptr(noise_c),
+                      noise_p=_ptr(noise_p), out_batch_stride=model_out.stride(0), n=n, hw=h * w,
+                      out_dtype=_dt(model_out.dtype), guided=int(bool(guided)), cfg_scale=cfg_scale, sigma=sigma,
+                      inv_alpha=1.0 / alpha, c_x=c_x, c_m0=c_m0, c_m1=c_m1, c_noise=c_noise, p_x=p_x, p_m0=p_m0,
+                      p_m1=p_m1, p_noise=p_noise)
+    _check(load().pxa_sa_solver_step(C.byref(args), _stream()), "pxa_sa_solver_step")
+    return x_pred
 
 
 # ------------------------------------------------------------------------------------------------- training backward

@@ -891,10 +891,12 @@ def install_into_reference() -> bool:
         setattr(nets, name, obj)
     nets.PixArtMSBlock = PixArtMSBlock
     nets.PixArtBlock = PixArtBlock
-    try:                                                   # the sampler the inference script imports from `diffusion`
+    try:                                                   # the samplers the inference script imports from `diffusion`
         import diffusion
+        from .sa_sampler import SASolverSampler
         from .sampler import DPMS
         diffusion.DPMS = DPMS
+        diffusion.SASolverSampler = SASolverSampler
     except Exception:
         pass
     return True

@@ -26,20 +26,65 @@ from . import lib
 __all__ = ["DPMS", "DPMSolverPP"]
 
 
+def linear_betas(diffusion_steps: int = 1000) -> np.ndarray:
+    """float64 linear beta schedule (diffusion/model/gaussian_diffusion.py:82,107-116)."""
+    scale = 1000 / diffusion_steps
+    return np.linspace(scale * 0.0001, scale * 0.02, diffusion_steps, dtype=np.float64)
+
+
+def _denoiser_params(model: Callable) -> list:
+    owner = getattr(model, "__self__", model)              # the nn.Module behind a bound forward_with_dpmsolver
+    return list(owner.parameters()) if isinstance(owner, torch.nn.Module) else []
+
+
+def _denoiser_key(model: Callable, params: list, model_kwargs: Optional[dict]) -> tuple:
+    """The denoiser's part of a captured sampling loop's cache key.  `model_kwargs` tensors are captured by address, and so
+    are the denoiser's parameters: the forward keeps derived copies (stacked kv_linear weights) a replay cannot refresh."""
+    kw_id = tuple(sorted((k, (v.data_ptr(), tuple(v.shape)) if isinstance(v, torch.Tensor) else repr(v))
+                         for k, v in (model_kwargs or {}).items()))
+    owner = getattr(model, "__self__", model)
+    derived = getattr(owner, "_kv_batch", None) is not None or getattr(owner, "_ln_fusion", None) is not None
+    wkey = (sum(p._version for p in params), params[0].data_ptr()) if (params and derived) else None
+    return kw_id, wkey
+
+
+def _capture(warmup: Callable[[], None], body: Callable[[], None]) -> torch.cuda.CUDAGraph:
+    """Run `warmup` eagerly on a side stream (lazy inits, tensor maps), then capture `body` into a CUDA graph."""
+    side = torch.cuda.Stream()
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        warmup()
+    torch.cuda.current_stream().wait_stream(side)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        body()
+    return graph
+
+
+def _step_input(out: torch.Tensor) -> torch.Tensor:
+    """The denoiser output as a step kernel reads it: fp32 or bf16 with dense (h, w) planes (channel slices are fine)."""
+    if out.dtype not in (torch.float32, torch.bfloat16):
+        out = out.float()
+    if not (out.stride(3) == 1 and out.stride(2) == out.shape[3] and out.stride(1) == out.shape[2] * out.shape[3]):
+        out = out.contiguous()
+    return out
+
+
 class _DiscreteVPSchedule:
     """log(alpha) of the discrete linear-beta VP schedule at t_i = i/N (float32 table, piecewise-linear look-up with the
     outermost segments extended), as `NoiseScheduleVP('discrete', betas=linear)` defines it
-    (diffusion/model/dpm_solver.py:97-106,127-155; betas: diffusion/model/gaussian_diffusion.py:82,107-116)."""
+    (diffusion/model/dpm_solver.py:97-106,127-155; betas: diffusion/model/gaussian_diffusion.py:82,107-116), or of a given
+    log(alpha) table at the same times (the SA-Solver's, diffusion/model/sa_solver.py:81-90)."""
 
-    def __init__(self, diffusion_steps: int = 1000, clipped_lambda: float = -5.1):
-        scale = 1000 / diffusion_steps
-        betas = np.linspace(scale * 0.0001, scale * 0.02, diffusion_steps, dtype=np.float64)
-        log_alphas = 0.5 * torch.log(1 - torch.from_numpy(betas)).cumsum(dim=0)
-        lambs = log_alphas - 0.5 * torch.log(1. - torch.exp(2. * log_alphas))
-        drop = int(torch.searchsorted(torch.flip(lambs, [0]), torch.tensor(clipped_lambda, dtype=lambs.dtype)))
-        if drop > 0:                       # log-SNR clipped near t = T (a no-op for the linear schedule)
-            log_alphas = log_alphas[:-drop]
-        self.log_alpha = log_alphas.to(torch.float32)
+    def __init__(self, diffusion_steps: int = 1000, clipped_lambda: float = -5.1, log_alpha: Optional[torch.Tensor] = None):
+        if log_alpha is None:
+            log_alphas = 0.5 * torch.log(1 - torch.from_numpy(linear_betas(diffusion_steps))).cumsum(dim=0)
+            lambs = log_alphas - 0.5 * torch.log(1. - torch.exp(2. * log_alphas))
+            drop = int(torch.searchsorted(torch.flip(lambs, [0]), torch.tensor(clipped_lambda, dtype=lambs.dtype)))
+            if drop > 0:                       # log-SNR clipped near t = T (a no-op for the linear schedule)
+                log_alphas = log_alphas[:-drop]
+            log_alpha = log_alphas
+        self.log_alpha = log_alpha.to(torch.float32)      # a given table is used as is: no clipping
         self.total_N = self.log_alpha.numel()
         self.t = torch.linspace(0., 1., self.total_N + 1)[1:].to(torch.float32)
         self.T = 1.0
@@ -74,8 +119,7 @@ class DPMSolverPP:
         self.schedule = _DiscreteVPSchedule(diffusion_steps)
         self._graphs: Dict[tuple, tuple] = {}
         self._cfg_cond: Optional[torch.Tensor] = None          # cat([uncondition, condition]), built once
-        owner = getattr(model, "__self__", model)              # the nn.Module behind a bound forward_with_dpmsolver
-        self._params = list(owner.parameters()) if isinstance(owner, torch.nn.Module) else []
+        self._params = _denoiser_params(model)
 
     # ---- host side: everything that does not depend on the latents
     def plan(self, steps: int, order: int = 2, t_start: Optional[float] = None, t_end: Optional[float] = None,
@@ -114,12 +158,8 @@ class DPMSolverPP:
             else:                                   # reference: a single conditional evaluation (dpm_solver.py:327-328)
                 out = self.model(x, t_in[:n], cond, **self.model_kwargs)
                 out = torch.cat([out, out])
-            if out.dtype not in (torch.float32, torch.bfloat16):
-                out = out.float()
-            if not (out.stride(3) == 1 and out.stride(2) == out.shape[3] and out.stride(1) == out.shape[2] * out.shape[3]):
-                out = out.contiguous()
-            lib.dpm_solver_pp_step(out, x, x0_prev, cfg_scale=self.cfg_scale if guided else 1.0, sigma_s=st["sigma_s"],
-                                   alpha_s=st["alpha_s"], a=st["a"], b=st["b"], c=st["c"])
+            lib.dpm_solver_pp_step(_step_input(out), x, x0_prev, cfg_scale=self.cfg_scale if guided else 1.0,
+                                   sigma_s=st["sigma_s"], alpha_s=st["alpha_s"], a=st["a"], b=st["b"], c=st["c"])
             if inter is not None:
                 inter.append(x.clone())
         return x
@@ -155,27 +195,18 @@ class DPMSolverPP:
     def _sample_graphed(self, x, plan, t_dev, cond):
         # every per-step scalar (sigma_s, alpha_s, a, b, c), the step orders and t_input are baked into the captured kernel
         # arguments, and `cond` / model_kwargs tensors into the captured forward: all of them are part of the key
-        kw_id = tuple(sorted((k, (v.data_ptr(), tuple(v.shape)) if isinstance(v, torch.Tensor) else repr(v))
-                             for k, v in (self.model_kwargs or {}).items()))
-        # ... and so are the denoiser's parameters: the forward keeps derived copies (stacked kv_linear weights) a replay cannot refresh
-        owner = getattr(self.model, "__self__", self.model)
-        derived = getattr(owner, "_kv_batch", None) is not None or getattr(owner, "_ln_fusion", None) is not None
-        wkey = (sum(p._version for p in self._params), self._params[0].data_ptr()) if (self._params and derived) else None
+        kw_id, wkey = _denoiser_key(self.model, self._params, self.model_kwargs)
         key = (tuple(x.shape), x.device.index, float(self.cfg_scale), cond.data_ptr(), tuple(cond.shape), kw_id, wkey,
                tuple((st["t_input"], st["sigma_s"], st["alpha_s"], st["a"], st["b"], st["c"], st.get("order")) for st in plan))
         if key not in self._graphs:
             x_static = x.to(torch.float32).contiguous().clone()
             x0_prev = torch.empty_like(x_static)
             z_in = torch.empty_like(x_static)
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):                      # warm-up outside capture (lazy inits, tensor maps)
-                self._run(x_static, x0_prev, plan[:2], t_dev[:2], cond, None)
-            torch.cuda.current_stream().wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
+
+            def body():
                 x_static.copy_(z_in)
                 self._run(x_static, x0_prev, plan, t_dev, cond, None)
+            graph = _capture(lambda: self._run(x_static, x0_prev, plan[:2], t_dev[:2], cond, None), body)
             self._graphs[key] = (graph, z_in, x_static, t_dev, cond)
         graph, z_in, x_static = self._graphs[key][:3]
         z_in.copy_(x)
