@@ -225,9 +225,10 @@ int pxa_groupnorm_silu_nhwc_bf16(const void* x, void* out, const void* gamma, co
                                  int32_t HW, int32_t C, int32_t groups, float eps, int32_t silu, void* stream);
 
 /* AdamW on a flat fp32 bucket (torch.optim.AdamW semantics: decoupled weight decay, bias-corrected moments) -- the optimizer
- * the reference trains with (configs/PixArt_xl2_internal.py:48 `AdamW(lr=2e-5, weight_decay=3e-2, eps=1e-10)`, built by
- * diffusion/utils/optimizer.py:236-245), applied to the gradient buckets of pixart_sigma_b200.parallel.GradBucketReducer in one
- * launch per bucket; optionally writes the bf16 copy of the updated parameters that the GEMMs read.  All pointers device. */
+ * of the PixArt-alpha configs (configs/PixArt_xl2_internal.py:48 `AdamW(lr=1e-4, weight_decay=3e-2, eps=1e-10)`, built by
+ * diffusion/utils/optimizer.py:236-245; the PixArt-Sigma configs train with CAME, pxa_came_flat below), applied to the
+ * gradient buckets of pixart_sigma_b200.parallel.GradBucketReducer in one launch per bucket; optionally writes the bf16 copy of
+ * the updated parameters that the GEMMs read.  All pointers device. */
 typedef struct PxaAdamWArgs {
   float* param;          /* fp32 [n], updated in place          */
   const float* grad;     /* fp32 [n]                            */
@@ -240,6 +241,81 @@ typedef struct PxaAdamWArgs {
   float grad_scale;      /* gradients are multiplied by this first (1 / loss scale, or 1) */
 } PxaAdamWArgs;
 int pxa_adamw_flat(const PxaAdamWArgs* args, void* stream);
+
+/* Gradient-norm clipping over flat gradient buckets (torch.nn.utils.clip_grad_norm_, which train_scripts/train.py:181-182
+ * reaches through accelerate):  g *= grad_scale;  total = ||g||_2 over every bucket;  g *= min(max_norm / (total + 1e-6), 1).
+ * Two launches: per-CTA partial sums of squares into `partials` (PXA_GRAD_CLIP_PARTS slots), then every CTA reduces the
+ * partials in the same fixed order, reads the coefficient on the device and scales its share.  No atomics, no host read:
+ * `total_norm` (fp32 0-d, device) receives the norm.  Bucket pointers are 16-byte aligned; the elements past `n` (padding)
+ * are not touched. */
+#define PXA_GRAD_CLIP_PARTS 1024
+#define PXA_GRAD_CLIP_MAX_BUCKETS 128
+typedef struct PxaGradBucket {
+  float* ptr;            /* fp32 [n], device, scaled in place */
+  int64_t n;
+} PxaGradBucket;
+typedef struct PxaGradClipArgs {
+  const PxaGradBucket* buckets;   /* HOST array [n_buckets] (passed to the kernels by value) */
+  int32_t n_buckets;              /* 1 .. PXA_GRAD_CLIP_MAX_BUCKETS */
+  float max_norm;
+  float grad_scale;               /* multiplied in first (1 / loss scale, or 1) */
+  float* partials;                /* fp32 [PXA_GRAD_CLIP_PARTS] workspace */
+  float* total_norm;              /* fp32 [1] out: the norm after grad_scale, before clipping */
+} PxaGradClipArgs;
+int pxa_grad_clip_flat(const PxaGradClipArgs* args, void* stream);
+
+/* CAME (came_pytorch.CAME.step, which every config under configs/pixart_sigma_config selects as `CAMEWrapper`,
+ * diffusion/utils/optimizer.py:242-246) over every parameter of every flat bucket.  Per parameter p with gradient g, no bias
+ * correction, state starting at zero:
+ *   u = g^2 + eps1;  factored (ndim >= 2, p viewed as `lead` matrices R x C):  row = b2 row + (1-b2) mean_C u,
+ *   col = b2 col + (1-b2) mean_R u,  u = rsqrt(row / mean_R row) rsqrt(col) g;   1-D:  v = b2 v + (1-b2) u,  u = rsqrt(v) g;
+ *   u /= max(RMS(u) / clip_threshold, 1);  m = b1 m + (1-b1) u;
+ *   factored: res = (u - m)^2 + eps2, rrow / rcol EMAs with b3 as above, upd = rsqrt(rrow / mean rrow) rsqrt(rcol) m;  1-D: upd = m;
+ *   p -= weight_decay * lr * p (if weight_decay != 0);  p -= lr * upd;  rms[e] = ||p_before||_2 / sqrt(numel).
+ * The parameter table (one PxaCameParam per parameter, built on the host and planned by pxa_came_workspace_bytes) is read
+ * from device memory, so one launch per pass covers every bucket: 7 launches per step whatever the bucket count.  Work is
+ * split into tiles: 2048 elements of a 1-D parameter; 256 whole matrices of a parameter whose matrices are at most 4 x 4 (one
+ * thread each); 128 x 128 blocks of a larger matrix, whose row / column partial sums go to the workspace and are reduced in
+ * a fixed order (no floating-point atomics: the same inputs give bitwise-equal results).  u is recomputed where needed,
+ * .grad is only read.  Parameters need no alignment (scalar coalesced accesses), the bucket padding is not touched.
+ * `lr` is read from device memory (a schedule can change it between CUDA-graph replays).  HBM-bound: 32 B per parameter
+ * (g read 4 times, exp_avg read + written, p read + written). */
+typedef struct PxaCameParam {
+  float* param;          /* device: the parameter's first element in its flat fp32 parameter bucket               */
+  const float* grad;     /* device: its gradient in the gradient bucket                                           */
+  float* exp_avg;        /* device: its first moment in the exp_avg bucket                                        */
+  int64_t numel;         /* lead * R * C                                                                          */
+  int64_t offset;        /* element offset of the parameter in its bucket ...                                     */
+  int64_t bucket_numel;  /* ... and the bucket's length: offset + numel <= bucket_numel is checked                */
+  int64_t sq_off;        /* factored: offset of its lead * R row statistics in sq_row / res_row;
+                            1-D: offset of its numel second moments in exp_avg_sq                                 */
+  int64_t col_off;       /* factored: offset of its lead * C column statistics in sq_col / res_col                */
+  int32_t lead, R, C;    /* 1-D: lead = 1, R = 1, C = numel                                                       */
+  int32_t factored;      /* 1: ndim >= 2                                                                          */
+  int64_t tile_begin;    /* plan, written by pxa_came_workspace_bytes: first tile ...                             */
+  int64_t fin_begin;     /* ... first statistics-finalisation work item ...                                       */
+  int64_t ws_off;        /* ... and workspace offset (floats) of the parameter                                    */
+} PxaCameParam;
+typedef struct PxaCameArgs {
+  const PxaCameParam* table;  /* DEVICE copy of the planned table [n_entries]                                     */
+  float* exp_avg_sq;          /* fp32 [n_vec]: second moments of the 1-D parameters                              */
+  float* sq_row; float* res_row;   /* fp32 [n_row]                                                                */
+  float* sq_col; float* res_col;   /* fp32 [n_col]                                                                */
+  float* rms;                 /* fp32 [n_entries] out                                                             */
+  const float* lr;            /* fp32 [1], device                                                                 */
+  void* workspace;            /* caller-owned, workspace_bytes >= what pxa_came_workspace_bytes returned          */
+  int64_t workspace_bytes;
+  int64_t n_vec, n_row, n_col;
+  int32_t n_entries;
+  int32_t step;               /* 1-based step count (CAME applies no bias correction; must be positive)           */
+  double eps1, eps2, clip_threshold, beta1, beta2, beta3, weight_decay;
+  int64_t n_tiles, n_fin, ws_floats;   /* plan totals, written by pxa_came_workspace_bytes                       */
+} PxaCameArgs;
+/* Checks every entry of the HOST table against `args` (shapes, bucket bounds, state offsets), writes its plan fields and
+ * args->n_tiles / n_fin / ws_floats, and returns the workspace size in *bytes.  Host only; call once, then copy the table
+ * to the device. */
+int pxa_came_workspace_bytes(PxaCameArgs* args, PxaCameParam* table_host, int64_t* bytes);
+int pxa_came_flat(const PxaCameArgs* args, void* stream);
 
 /* ------------------------------------------------------------------------------------------- attention
  * out[b, i, h, :] = softmax_j( q[b,i,h,:] . k[b,j,h,:] * scale ) v[b,j,h,:],  j < kv_len[b],  head_dim 72.

@@ -714,8 +714,9 @@ namespace pxa {
 // ------------------------------------------------------------------------------------------------- AdamW on a flat bucket
 // One elementwise pass over a flat fp32 (parameter, gradient, exp_avg, exp_avg_sq) bucket -- torch.optim.AdamW's update
 // (decoupled weight decay, bias corrections folded into two host-computed scalars) -- optionally emitting the bf16 weight
-// copy the GEMMs read.  The reference trains with AdamW(lr 2e-5, weight_decay 3e-2, eps 1e-10)
-// (configs/PixArt_xl2_internal.py:48; diffusion/utils/optimizer.py:236-245 build_optimizer).  HBM-bound: 16 B read + 12 B
+// copy the GEMMs read.  The PixArt-alpha configs train with AdamW(lr 1e-4, weight_decay 3e-2, eps 1e-10)
+// (configs/PixArt_xl2_internal.py:48; diffusion/utils/optimizer.py:236-245 build_optimizer); the PixArt-Sigma configs use
+// CAME (optim_sm90.cu).  HBM-bound: 16 B read + 12 B
 // (+ 2 B) written per parameter.
 __global__ void __launch_bounds__(256) adamw_flat_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                          float* __restrict__ v, __nv_bfloat16* __restrict__ shadow, long long n4,

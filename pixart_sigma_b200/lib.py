@@ -60,6 +60,33 @@ class AdamWArgs(C.Structure):
                 ("beta2", C.c_float), ("eps", C.c_float), ("weight_decay", C.c_float), ("grad_scale", C.c_float)]
 
 
+GRAD_CLIP_PARTS, GRAD_CLIP_MAX_BUCKETS = 1024, 128
+
+
+class GradBucket(C.Structure):
+    _fields_ = [("ptr", C.c_void_p), ("n", C.c_int64)]
+
+
+class GradClipArgs(C.Structure):
+    _fields_ = [("buckets", C.POINTER(GradBucket)), ("n_buckets", C.c_int32), ("max_norm", C.c_float), ("grad_scale", C.c_float),
+                ("partials", C.c_void_p), ("total_norm", C.c_void_p)]
+
+
+class CameParam(C.Structure):
+    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("numel", C.c_int64), ("offset", C.c_int64),
+                ("bucket_numel", C.c_int64), ("sq_off", C.c_int64), ("col_off", C.c_int64), ("lead", C.c_int32), ("R", C.c_int32),
+                ("C", C.c_int32), ("factored", C.c_int32), ("tile_begin", C.c_int64), ("fin_begin", C.c_int64), ("ws_off", C.c_int64)]
+
+
+class CameArgs(C.Structure):
+    _fields_ = [("table", C.c_void_p), ("exp_avg_sq", C.c_void_p), ("sq_row", C.c_void_p), ("res_row", C.c_void_p),
+                ("sq_col", C.c_void_p), ("res_col", C.c_void_p), ("rms", C.c_void_p), ("lr", C.c_void_p), ("workspace", C.c_void_p),
+                ("workspace_bytes", C.c_int64), ("n_vec", C.c_int64), ("n_row", C.c_int64), ("n_col", C.c_int64),
+                ("n_entries", C.c_int32), ("step", C.c_int32), ("eps1", C.c_double), ("eps2", C.c_double),
+                ("clip_threshold", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double), ("beta3", C.c_double),
+                ("weight_decay", C.c_double), ("n_tiles", C.c_int64), ("n_fin", C.c_int64), ("ws_floats", C.c_int64)]
+
+
 class LnModArgs(C.Structure):
     _fields_ = [("x", C.c_void_p), ("out", C.c_void_p), ("shift", C.c_void_p), ("scale", C.c_void_p),
                 ("mod_batch_stride", C.c_int64), ("rows_per_batch", C.c_int32),
@@ -149,7 +176,8 @@ EXPORTS = ("pxa_transpose_bf16", "pxa_gelu_tanh_bf16", "pxa_gate_residual_fwd", 
            "pxa_version", "pxa_last_error", "pxa_launch_count", "pxa_gemm_bf16", "pxa_ln_modulate",
            "pxa_flash_attn_d72_bf16", "pxa_kv_compress_conv2_ln", "pxa_conv3x3_nhwc_bf16", "pxa_dpm_solver_pp_step",
            "pxa_ln_prepare", "pxa_layernorm_affine_bf16", "pxa_groupnorm_silu_nhwc_bf16", "pxa_adamw_flat", "pxa_mlp_fused_bf16",
-           "pxa_rmsnorm_bf16", "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step")
+           "pxa_rmsnorm_bf16", "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step",
+           "pxa_grad_clip_flat", "pxa_came_workspace_bytes", "pxa_came_flat")
 
 _lib = None
 
@@ -169,7 +197,8 @@ def load() -> C.CDLL:
                              ("pxa_conv3x3_nhwc_bf16", Conv3x3Args), ("pxa_dpm_solver_pp_step", DpmStepArgs),
                              ("pxa_ln_prepare", LnPrepareArgs), ("pxa_adamw_flat", AdamWArgs),
                              ("pxa_mlp_fused_bf16", MlpArgs), ("pxa_t5_attn_d64_bf16", T5AttnArgs),
-                             ("pxa_sa_solver_step", SaStepArgs)):
+                             ("pxa_sa_solver_step", SaStepArgs), ("pxa_grad_clip_flat", GradClipArgs),
+                             ("pxa_came_flat", CameArgs)):
             fn = getattr(lib, name)
             fn.restype = C.c_int
             fn.argtypes = [C.POINTER(struct), C.c_void_p]
@@ -179,6 +208,8 @@ def load() -> C.CDLL:
             fn = getattr(lib, name)
             fn.restype = C.c_int
             fn.argtypes = [C.POINTER(struct), C.c_void_p]
+        lib.pxa_came_workspace_bytes.restype = C.c_int
+        lib.pxa_came_workspace_bytes.argtypes = [C.POINTER(CameArgs), C.POINTER(CameParam), C.POINTER(C.c_int64)]
         lib.pxa_layernorm_affine_bf16.restype = C.c_int
         lib.pxa_layernorm_affine_bf16.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_float,
                                                   C.c_void_p]
@@ -437,6 +468,44 @@ def adamw_flat(param: torch.Tensor, grad: torch.Tensor, exp_avg: torch.Tensor, e
                      n=param.numel(), step=step, lr=lr, beta1=betas[0], beta2=betas[1], eps=eps, weight_decay=weight_decay,
                      grad_scale=grad_scale)
     _check(load().pxa_adamw_flat(C.byref(args), _stream()), "pxa_adamw_flat")
+
+
+def grad_clip_flat(grads, partials: torch.Tensor, total_norm: torch.Tensor, *, max_norm: float, grad_scale: float = 1.0,
+                   lengths=None) -> torch.Tensor:
+    """torch.nn.utils.clip_grad_norm_ over flat fp32 gradient buffers, in place (include/pixart_sm100.h: pxa_grad_clip_flat):
+    g *= grad_scale, total = ||g||, g *= min(max_norm / (total + 1e-6), 1).  `lengths[k]`: elements of grads[k] that belong to
+    a parameter (default: all).  partials: fp32 [GRAD_CLIP_PARTS] workspace; total_norm (fp32, 1 element) receives the norm on
+    the device."""
+    grads = list(grads)
+    lengths = [g.numel() for g in grads] if lengths is None else list(lengths)
+    for g, n in zip(grads, lengths):
+        if not (g.is_cuda and g.dtype == torch.float32 and g.is_contiguous() and 0 < n <= g.numel()):
+            raise PxaError("grad_clip_flat: gradients must be contiguous fp32 CUDA tensors")
+    for t in (partials, total_norm):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+            raise PxaError("grad_clip_flat: partials / total_norm must be contiguous fp32 CUDA tensors")
+    if partials.numel() < GRAD_CLIP_PARTS or total_norm.numel() != 1:
+        raise PxaError(f"grad_clip_flat: partials needs {GRAD_CLIP_PARTS} elements, total_norm 1")
+    arr = (GradBucket * max(len(grads), 1))(*[GradBucket(ptr=g.data_ptr(), n=n) for g, n in zip(grads, lengths)])
+    args = GradClipArgs(buckets=arr, n_buckets=len(grads), max_norm=max_norm, grad_scale=grad_scale, partials=_ptr(partials),
+                        total_norm=_ptr(total_norm))
+    _check(load().pxa_grad_clip_flat(C.byref(args), _stream()), "pxa_grad_clip_flat")
+    return total_norm
+
+
+def came_plan(args: CameArgs, table) -> int:
+    """Validate and plan the host parameter table (a ctypes array of CameParam) in place; fills args.n_tiles / n_fin /
+    ws_floats and returns the workspace size in bytes (include/pixart_sm100.h: pxa_came_workspace_bytes)."""
+    nbytes = C.c_int64(0)
+    args.n_entries = len(table)
+    _check(load().pxa_came_workspace_bytes(C.byref(args), table, C.byref(nbytes)), "pxa_came_workspace_bytes")
+    return int(nbytes.value)
+
+
+def came_flat(args: CameArgs) -> None:
+    """One CAME step over every parameter of a planned table (include/pixart_sm100.h: pxa_came_flat); `args` holds raw
+    device pointers, so the caller keeps the tensors behind them alive."""
+    _check(load().pxa_came_flat(C.byref(args), _stream()), "pxa_came_flat")
 
 
 def groupnorm_silu_nhwc(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, out: torch.Tensor, *, groups: int = 32,
