@@ -60,7 +60,11 @@ uint64_t pxa_launch_count(void);
  *   = rstd_r * ( acc[r,n] - mu_r * u_b[n] ) + v_b[n],     acc = A W^T,  A[r,k] = bf16( x[r,k] (1 + scale_b[k]) ),
  *     u_b[n] = sum_k (1 + scale_b[k]) W[n,k],   v_b[n] = sum_k shift_b[k] W[n,k] + bias[n].
  * A and the per-row statistics are by-products of the residual epilogue that produced x (`aux_scale`, `row_stats_out`
- * below) or of pxa_ln_prepare; u_b / v_b are two tiny per-sample GEMVs per forward. */
+ * below) or of pxa_ln_prepare; u_b / v_b are two tiny per-sample GEMVs per forward.
+ * Accuracy trade-off: A is rounded to bf16 relative to |x|, not to the normalised x - mu, and the row variance comes from
+ * one-pass fp32 sums.  The error against the unfused LayerNorm therefore grows like 1 + |mu_r| rstd_r (about
+ * 2^-9 rstd sum_k |x_k (1 + scale_k) W[n,k]| at worst, tests/test_numerics_gpu.py); the unfused pxa_ln_modulate path
+ * (two-pass statistics, the default) has no such dependence on the mean. */
 #define PXA_EPI_LN_BIAS 5       /* out = rstd*(acc - mu*u) + v            (`ln_*` fields; bias must be NULL: it is inside v) */
 #define PXA_EPI_LN_BIAS_GELU 6  /* out = gelu_tanh(rstd*(acc - mu*u) + v)                                                   */
 #define PXA_LN_STAT_PARTS 8     /* row statistics are kept as 8 partial (sum x, sum x^2) pairs per row: fp32 [M][8][2]      */

@@ -556,8 +556,18 @@ namespace pxa {
 // reference call site scripts/inference.py:136).  Two passes over an NHWC bf16 image: (1) per (sample, group) sum / sum of
 // squares -- each thread walks pixels for a fixed 8-channel slice, CTA-level reduction in smem, one atomic per group and
 // CTA; (2) y = silu((x - mean_g) rstd_g gamma_c + beta_c).  Algorithmic bytes: 2 reads + 1 write of the image (6 B/element).
+// The sums are taken over x - K_g, where the pivot K_g is the (sample, group)'s first element (pixel 0, first channel of the
+// group): the one-pass variance E[x^2] - mean^2 would otherwise cancel when |mean| / std is large (at 128 it loses every
+// significant bit of a 4 M-element group in fp32).  stats therefore holds the sums of x - K_g, and the apply pass re-reads K_g.
 constexpr int kGnThreads = 256;
 constexpr int kGnMaxGroups = 64;
+
+// The pivots of the 8 channels c0 .. c0 + 7 of sample b (one bf16 load per channel, L1/L2 resident).
+PXA_DEVICE void gn_pivots(float (&k)[8], const __nv_bfloat16* x, int b, int HW, int C, int cpg, int c0) {
+  const __nv_bfloat16* p = x + (size_t)b * HW * C;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) k[i] = __bfloat162float(p[((c0 + i) / cpg) * cpg]);
+}
 
 __global__ void __launch_bounds__(kGnThreads) gn_stats_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ stats,
                                                               int HW, int C, int groups, int pix_per_cta) {
@@ -570,10 +580,11 @@ __global__ void __launch_bounds__(kGnThreads) gn_stats_kernel(const __nv_bfloat1
   __syncthreads();
   const int p0 = blockIdx.x * pix_per_cta;
   const int p1 = min(p0 + pix_per_cta, HW);
-  float s[8], q[8];
+  float s[8], q[8], piv[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) s[i] = q[i] = 0.f;
   if (prow < prows) {
+    gn_pivots(piv, x, b, HW, C, cpg, slice * 8);
     const __nv_bfloat16* base = x + ((size_t)b * HW) * C + slice * 8;
 #pragma unroll 4
     for (int p = p0 + prow; p < p1; p += prows) {
@@ -581,7 +592,7 @@ __global__ void __launch_bounds__(kGnThreads) gn_stats_kernel(const __nv_bfloat1
       const uint32_t w[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        const float a = bf16_lo(w[i]), c = bf16_hi(w[i]);
+        const float a = bf16_lo(w[i]) - piv[2 * i], c = bf16_hi(w[i]) - piv[2 * i + 1];
         s[2 * i] += a; q[2 * i] = fmaf(a, a, q[2 * i]);
         s[2 * i + 1] += c; q[2 * i + 1] = fmaf(c, c, q[2 * i + 1]);
       }
@@ -630,12 +641,14 @@ __global__ void __launch_bounds__(kGnThreads) gn_apply_kernel(const __nv_bfloat1
     }
   }
   int b_prev = -1;
-  float a[8], d[8];                                                // y = x * a + d  with a = rstd * gamma, d = beta - mean * a
+  // y = (x - K) * a + d  with a = rstd * gamma, d = beta - mean * a, mean = the mean of x - K (K: the pivots, see above)
+  float a[8], d[8], piv[8];
   for (long long i = i0; i < total_slices; i += (long long)gridDim.x * kGnThreads) {
     const long long pix = i / slices;                              // b * HW + p
     const int b = (int)(pix / HW);
     if (b != b_prev) {                                             // new sample: fold its group statistics into (a, d)
       b_prev = b;
+      gn_pivots(piv, x, b, HW, C, cpg, c0);
       int g_prev = -1;
       float mean = 0.f, rstd = 0.f;
 #pragma unroll
@@ -656,8 +669,8 @@ __global__ void __launch_bounds__(kGnThreads) gn_apply_kernel(const __nv_bfloat1
     uint32_t o[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      float y0 = fmaf(bf16_lo(w[k]), a[2 * k], d[2 * k]);
-      float y1 = fmaf(bf16_hi(w[k]), a[2 * k + 1], d[2 * k + 1]);
+      float y0 = fmaf(bf16_lo(w[k]) - piv[2 * k], a[2 * k], d[2 * k]);
+      float y1 = fmaf(bf16_hi(w[k]) - piv[2 * k + 1], a[2 * k + 1], d[2 * k + 1]);
       if (kSilu) {
         y0 = __fdividef(y0, 1.0f + __expf(-y0));
         y1 = __fdividef(y1, 1.0f + __expf(-y1));

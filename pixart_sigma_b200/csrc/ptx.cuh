@@ -290,26 +290,36 @@ PXA_DEVICE float fast_exp2(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
   return y;
 }
-PXA_DEVICE float fast_tanh(float x) {
+PXA_DEVICE float fast_rcp(float x) {
   float y;
-  asm("tanh.approx.f32 %0, %1;\n" : "=f"(y) : "f"(x));
+  asm("rcp.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
   return y;
 }
-// GELU(approximate='tanh'): 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3)))
+// GELU(approximate='tanh'): 0.5 x (1 + tanh(u)), u = sqrt(2/pi) (x + 0.044715 x^3), evaluated as x * s with
+// s = sigmoid(2u) = 1 / (1 + e), e = exp(-2u).  The two forms are equal, but 1 + tanh(u) cancels for x below about -1.5,
+// where the 2^-11 error bound of tanh.approx becomes the whole result; here every factor keeps its relative accuracy
+// (ex2.approx and rcp.approx are good to about 2^-22), so the result is within 1 bf16 ulp wherever |gelu(x)| > 2^-40.
 PXA_DEVICE float gelu_tanh(float x) {
-  const float k0 = 0.7978845608028654f, k1 = 0.044715f;
-  float u = k0 * x * fmaf(k1 * x, x, 1.0f);
-  return 0.5f * x * (1.0f + fast_tanh(u));
+  const float k0 = 0.7978845608028654f, k1 = 0.044715f, m2log2e = -2.0f * 1.4426950408889634f;
+  const float u = k0 * x * fmaf(k1 * x, x, 1.0f);
+  return x * fast_rcp(1.0f + fast_exp2(m2log2e * u));
 }
 
-// d/dx gelu_tanh(x)  (same tanh.approx as the forward)
+// d/dx gelu_tanh(x) = s (1 + 2 x (1 - s) u') in the same sigmoid form, with 1 - s = e s (no cancellation as s -> 1).
+// e s is capped at 1: for x below about -9.4, e overflows to inf and s to 0, and the derivative is s (...) = 0.  x is clamped
+// to [-100, 100], where the fp32 derivative is already exactly 0 / 1 and no intermediate overflows; +-inf and NaN give NaN,
+// as torch's gelu backward does.
 PXA_DEVICE float gelu_tanh_grad(float x) {
-  const float k0 = 0.7978845608028654f, k1 = 0.044715f;
-  const float x2 = x * x;
-  const float u = k0 * x * fmaf(k1, x2, 1.0f);
-  const float t = fast_tanh(u);
+  const float k0 = 0.7978845608028654f, k1 = 0.044715f, m2log2e = -2.0f * 1.4426950408889634f;
+  const float xc = fminf(fmaxf(x, -100.0f), 100.0f);
+  const float x2 = xc * xc;
+  const float u = k0 * xc * fmaf(k1, x2, 1.0f);
   const float du = k0 * fmaf(3.0f * k1, x2, 1.0f);
-  return 0.5f * (1.0f + t) + 0.5f * x * (1.0f - t * t) * du;
+  const float e = fast_exp2(m2log2e * u);
+  const float s = fast_rcp(1.0f + e);
+  const float es = fminf(e * s, 1.0f);
+  const float g = s * fmaf(2.0f * xc * es, du, 1.0f);
+  return fabsf(x) < INFINITY ? g : x - x;
 }
 
 }  // namespace pxa
