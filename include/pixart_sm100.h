@@ -451,6 +451,121 @@ typedef struct PxaSaStepArgs {
 } PxaSaStepArgs;
 int pxa_sa_solver_step(const PxaSaStepArgs* args, void* stream);
 
+/* ------------------------------------------------------------------------------------ LCM sampler step
+ * One step of the reference's 4-step LCM sampler (`LCMScheduler.step`, diffusion/lcm_scheduler.py:310-410, epsilon
+ * prediction; loop: train_scripts/train_pixart_lcm.py:105-135) in one elementwise pass:
+ *     x0       = (x - sqrt_beta * eps) / sqrt_alpha            (sqrt(1 - ac_t), sqrt(ac_t))
+ *     denoised = c_out * x0 + c_skip * x
+ *     x_next   = c_prev * denoised + c_noise * noise           (sqrt(ac_prev), sqrt(1 - ac_prev); 1-step: c_prev = 1, c_noise = 0)
+ * Every scalar comes from the host plan (float32 values computed with the reference's float32 torch operations).  Each
+ * product, sum and the division is rounded separately (no FMA contraction), which is the reference's sequence of fp32
+ * tensor operations.  `noise` is not read when c_noise == 0 (it may be NULL).  eps is `model_out` channels 0..3 (a
+ * channel slice of the 8-channel learn-sigma output is fine), fp32 or bf16.  x, noise, denoised, x_next: fp32
+ * [n, 4, hw] contiguous; x_next may alias x.  HBM-bound: 20 (bf16 eps, no noise) .. 28 algorithmic bytes per element. */
+typedef struct PxaLcmStepArgs {
+  const void* model_out;    /* [n, >=4, hw], dtype out_dtype, sample b at b * out_batch_stride              */
+  const float* x;           /* fp32 [n, 4, hw]: the sample at t                                              */
+  const float* noise;       /* fp32 [n, 4, hw], or NULL when c_noise == 0                                    */
+  float* denoised;          /* fp32 [n, 4, hw] out                                                           */
+  float* x_next;            /* fp32 [n, 4, hw] out (may alias x)                                             */
+  int64_t out_batch_stride; /* elements                                                                      */
+  int32_t n, hw;
+  int32_t out_dtype;        /* PXA_DTYPE_*                                                                   */
+  float sqrt_alpha, sqrt_beta, c_skip, c_out, c_prev, c_noise;
+} PxaLcmStepArgs;
+int pxa_lcm_step(const PxaLcmStepArgs* args, void* stream);
+
+/* ------------------------------------------------------------------------------------ LCM consistency distillation
+ * The per-step glue of train_scripts/train_pixart_lcm.py:223-303 (IDDPM with return_startx, DDIMSolver, boundary
+ * scalings) as two kernels over a device table of PXA_LCM_MAX_ROWS rows, one per DDIM index (num_ddim_timesteps rows,
+ * uploaded once and indexed on the device by `index`, so a step never reads anything back to the host):
+ *   start = ddim_timesteps[index], t = max(start - k, 0) with k = train_timesteps / num_ddim_timesteps
+ *   row.sra_s, row.srm1_s   = fp32 sqrt(1 / ac[start]), sqrt(1 / ac[start] - 1)      (IDDPM's fp64 tables, rounded)
+ *   row.cskip_s, row.cout_s = the fp32 boundary scalings at start (scalings_for_boundary_conditions on int64 steps)
+ *   row.sra_t .. row.cout_t = the same at t
+ *   row.sqrt_acp, row.sqrt_1macp = fp64 sqrt(ac_prev[index]), sqrt(1 - ac_prev[index])  (DDIMSolver.ddim_alpha_cumprods_prev)
+ * An index outside [0, n_rows) gives NaN for that sample. */
+#define PXA_LCM_MAX_ROWS 1000
+#define PXA_LCM_LOSS_PARTS 512
+#define PXA_LCM_HUBER 0
+#define PXA_LCM_L2 1
+typedef struct PxaLcmRow {
+  float sra_s, srm1_s, cskip_s, cout_s;
+  float sra_t, srm1_t, cskip_t, cout_t;
+  double sqrt_acp, sqrt_1macp;
+} PxaLcmRow;
+
+/* pxa_lcm_teacher_target: guided DDIM target from the teacher's batch-2b output [cond (b) ; uncond (b)] at x_t:
+ *     x0_c = sra_s x_t - srm1_s eps_c,   x0_u = sra_s x_t - srm1_s eps_u                  (fp32, as the reference)
+ *     x0   = x0_c + w (x0_c - x0_u),     eps = eps_c + w (eps_c - eps_u)                  (fp32, as the reference)
+ *     x_prev = fp32( sqrt_acp * x0 + sqrt_1macp * eps )                                     (fp64 products and sum)
+ * The reference's DDIM step multiplies by fp64 (b,1,1,1) tables, so its x_prev is fp64 and is rounded to fp32 only where
+ * it is used (`x_prev.float()`, the loss).  Here that step is evaluated in fp64 with the same fp64 coefficients and
+ * rounded once, so x_prev equals the reference's `x_prev.float()` exactly for the same fp32 x0 and eps.  The one place the
+ * reference keeps more: its target uses the fp64 x_prev (c_skip(t) x_prev), the loss kernel the fp32 one (a relative
+ * difference of at most 2^-24 in that term).  teacher_out: fp32 or bf16, channel slices fine; x_t, x_prev fp32 [b, 4, hw]. */
+typedef struct PxaLcmTeacherArgs {
+  const void* teacher_out;  /* [2b, >=4, hw], dtype out_dtype, sample r at r * out_batch_stride              */
+  const float* x_t;         /* fp32 [b, 4, hw]                                                               */
+  const int64_t* index;     /* DEVICE [b] DDIM indices                                                       */
+  const PxaLcmRow* table;   /* DEVICE [n_rows]                                                               */
+  float* x_prev;            /* fp32 [b, 4, hw] out                                                           */
+  int64_t out_batch_stride;
+  int32_t b, hw, out_dtype, n_rows;
+  float w;                  /* guidance scale (config cfg_scale)                                             */
+} PxaLcmTeacherArgs;
+int pxa_lcm_teacher_target(const PxaLcmTeacherArgs* args, void* stream);
+
+/* pxa_lcm_consistency_loss: the consistency loss and its gradient with respect to the student's output, per element
+ *     model_pred = cskip_s x_t + cout_s (sra_s x_t - srm1_s eps_s)                         (fp32, as the reference)
+ *     target     = fp32( cskip_t x_prev + fp32(cout_t (sra_t x_prev - srm1_t eps_e)) )     (fp64 sum, as the reference)
+ *     d = model_pred - target;   huber: l = sqrt(d^2 + c^2) - c, evaluated as d^2 / (sqrt(d^2 + c^2) + c) (no cancellation
+ *     for |d| << c);  l2: l = d^2
+ *     loss = mean(l) over b * 4 * hw  ->  *loss (fp32)
+ *     d_student_out[:, 0:4] = dl/dd * (-cout_s srm1_s) / (b * 4 * hw),   d_student_out[:, 4:out_channels] = 0 exactly
+ * Launch 1: one pass over the elements by PXA_LCM_LOSS_PARTS CTAs, each writing the fp64 sum of its elements' l to
+ * partials[cta]; launch 2: one CTA sums the partials in index order.  No floating-point atomics: the result is bitwise
+ * reproducible.  eps_s: fp32 (the student's output); eps_e: fp32 or bf16; both channel slices of [*, >=4, hw] outputs. */
+typedef struct PxaLcmLossArgs {
+  const float* student_out;   /* fp32 [b, >=4, hw], sample b at b * student_batch_stride                     */
+  const void* ema_out;        /* [b, >=4, hw], dtype ema_dtype, sample b at b * ema_batch_stride               */
+  const float* x_t;           /* fp32 [b, 4, hw]                                                             */
+  const float* x_prev;        /* fp32 [b, 4, hw]                                                             */
+  const int64_t* index;       /* DEVICE [b]                                                                  */
+  const PxaLcmRow* table;     /* DEVICE [n_rows]                                                             */
+  float* d_student_out;       /* fp32 [b, out_channels, hw] contiguous out                                   */
+  float* loss;                /* fp32 [1] out                                                                */
+  double* partials;           /* fp64 [PXA_LCM_LOSS_PARTS] workspace                                         */
+  int64_t student_batch_stride, ema_batch_stride;
+  int32_t b, hw, ema_dtype, n_rows;
+  int32_t out_channels;       /* 4 or 8                                                                      */
+  int32_t loss_type;          /* PXA_LCM_HUBER or PXA_LCM_L2                                                 */
+  float huber_c;
+} PxaLcmLossArgs;
+int pxa_lcm_consistency_loss(const PxaLcmLossArgs* args, void* stream);
+
+/* ------------------------------------------------------------------------------------ flat EMA update
+ * ema_update(model_ema, model, rate) of train_scripts/train_pixart_lcm.py:48-53 (`d.mul_(rate).add_((1 - rate) * s)`) over
+ * every bucket in ONE launch (grid: x = CTAs per bucket, y = bucket), reading a DEVICE table of buckets:
+ *     master[i] = fp32(fp32(master[i] * rate) + fp32(src[i] * (1 - rate)))      (three roundings, no FMA: bitwise torch's)
+ *     shadow[i] = bf16(master[i])                                                 (round to nearest even)
+ * for i < n only: the padding of a bucket is never read or written.  rate and 1 - rate are rounded to fp32 from the double
+ * `rate` as torch does for a Python scalar.  master, src: 16-byte aligned; shadow: 8-byte aligned.  14 B of HBM traffic
+ * per parameter (read 4 + 4, write 4 + 2). */
+typedef struct PxaEmaBucket {
+  float* master;            /* fp32 [n] EMA master values, in / out                                          */
+  const float* src;         /* fp32 [n] the online model's parameters                                        */
+  void* shadow;             /* bf16 [n] out: the EMA model's forward weights (NULL: not written)             */
+  int64_t n;                /* parameter elements of the bucket (its padding excluded)                       */
+} PxaEmaBucket;
+typedef struct PxaEmaArgs {
+  const PxaEmaBucket* table;  /* DEVICE [n_buckets]                                                         */
+  int32_t n_buckets;          /* 1 .. 65535                                                                  */
+  int64_t max_n;              /* max over the buckets of n (sizes the grid)                                  */
+  double rate;
+} PxaEmaArgs;
+int pxa_ema_flat(const PxaEmaArgs* args, void* stream);
+
 /* =============================================================================================== training backward
  * The reference trains through torch autograd (train_scripts/train.py:197 `accelerator.backward(loss)`, per-block
  * activation checkpointing diffusion/model/utils.py:28-45).  The entry points below are the backward twins of the forward

@@ -7,6 +7,8 @@ Only what the path `PixArtMS.forward -> 28 x PixArtMSBlock.forward` needs:
   sampler.py DPM-Solver++ loop around the path (mirror of the reference's `diffusion.DPMS`), fused step kernel + CUDA graph
   sa_sampler.py  SA-Solver loop (mirror of the reference's `diffusion.SASolverSampler`), fused predictor-corrector step
              kernel + CUDA graph
+  lcm.py     LCM: the few-step sampler (mirror of the reference's `LCMScheduler` loop) and consistency distillation with a
+             fused flat EMA update
   autograd.py / training.py  training path: the block's ops as autograd Functions over forward + backward kernels, IDDPM loss
   parallel.py  batch-sharded inference replicas; bucketed gradient all-reduce for data-parallel training
   vae.py / t5.py  the callers either side of the path on the same kernels: SDXL-VAE (diffusers' AutoencoderKL layout) and the
@@ -15,6 +17,7 @@ Only what the path `PixArtMS.forward -> 28 x PixArtMSBlock.forward` needs:
 """
 from .model import (MODELS, PixArt, PixArt_XL_2, PixArtBlock, PixArtMS, PixArtMS_XL_2, PixArtMSBlock,  # noqa: F401
                     build_model, install_into_reference, set_grad_checkpoint)
+from .lcm import LCMDistiller, LCMSampler, LCMScheduler  # noqa: F401
 from .sa_sampler import SASolverSampler  # noqa: F401
 from .sampler import DPMS, DPMSolverPP  # noqa: F401
 

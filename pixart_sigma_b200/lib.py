@@ -140,6 +140,45 @@ class SaStepArgs(C.Structure):
                 ("p_x", C.c_float), ("p_m0", C.c_float), ("p_m1", C.c_float), ("p_noise", C.c_float)]
 
 
+class LcmStepArgs(C.Structure):
+    _fields_ = [("model_out", C.c_void_p), ("x", C.c_void_p), ("noise", C.c_void_p), ("denoised", C.c_void_p),
+                ("x_next", C.c_void_p), ("out_batch_stride", C.c_int64), ("n", C.c_int32), ("hw", C.c_int32),
+                ("out_dtype", C.c_int32), ("sqrt_alpha", C.c_float), ("sqrt_beta", C.c_float), ("c_skip", C.c_float),
+                ("c_out", C.c_float), ("c_prev", C.c_float), ("c_noise", C.c_float)]
+
+
+LCM_MAX_ROWS, LCM_LOSS_PARTS = 1000, 512
+LCM_HUBER, LCM_L2 = 0, 1
+
+
+class LcmRow(C.Structure):
+    _fields_ = [("sra_s", C.c_float), ("srm1_s", C.c_float), ("cskip_s", C.c_float), ("cout_s", C.c_float),
+                ("sra_t", C.c_float), ("srm1_t", C.c_float), ("cskip_t", C.c_float), ("cout_t", C.c_float),
+                ("sqrt_acp", C.c_double), ("sqrt_1macp", C.c_double)]
+
+
+class LcmTeacherArgs(C.Structure):
+    _fields_ = [("teacher_out", C.c_void_p), ("x_t", C.c_void_p), ("index", C.c_void_p), ("table", C.c_void_p),
+                ("x_prev", C.c_void_p), ("out_batch_stride", C.c_int64), ("b", C.c_int32), ("hw", C.c_int32),
+                ("out_dtype", C.c_int32), ("n_rows", C.c_int32), ("w", C.c_float)]
+
+
+class LcmLossArgs(C.Structure):
+    _fields_ = [("student_out", C.c_void_p), ("ema_out", C.c_void_p), ("x_t", C.c_void_p), ("x_prev", C.c_void_p),
+                ("index", C.c_void_p), ("table", C.c_void_p), ("d_student_out", C.c_void_p), ("loss", C.c_void_p),
+                ("partials", C.c_void_p), ("student_batch_stride", C.c_int64), ("ema_batch_stride", C.c_int64),
+                ("b", C.c_int32), ("hw", C.c_int32), ("ema_dtype", C.c_int32), ("n_rows", C.c_int32),
+                ("out_channels", C.c_int32), ("loss_type", C.c_int32), ("huber_c", C.c_float)]
+
+
+class EmaBucket(C.Structure):
+    _fields_ = [("master", C.c_void_p), ("src", C.c_void_p), ("shadow", C.c_void_p), ("n", C.c_int64)]
+
+
+class EmaArgs(C.Structure):
+    _fields_ = [("table", C.c_void_p), ("n_buckets", C.c_int32), ("max_n", C.c_int64), ("rate", C.c_double)]
+
+
 class GateResidualArgs(C.Structure):
     _fields_ = [("x", C.c_void_p), ("y", C.c_void_p), ("gate", C.c_void_p), ("out", C.c_void_p), ("dgate", C.c_void_p),
                 ("gate_batch_stride", C.c_int64), ("rows_per_batch", C.c_int32), ("M", C.c_int32), ("C", C.c_int32)]
@@ -177,7 +216,8 @@ EXPORTS = ("pxa_transpose_bf16", "pxa_gelu_tanh_bf16", "pxa_gate_residual_fwd", 
            "pxa_flash_attn_d72_bf16", "pxa_kv_compress_conv2_ln", "pxa_conv3x3_nhwc_bf16", "pxa_dpm_solver_pp_step",
            "pxa_ln_prepare", "pxa_layernorm_affine_bf16", "pxa_groupnorm_silu_nhwc_bf16", "pxa_adamw_flat", "pxa_mlp_fused_bf16",
            "pxa_rmsnorm_bf16", "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step",
-           "pxa_grad_clip_flat", "pxa_came_workspace_bytes", "pxa_came_flat")
+           "pxa_grad_clip_flat", "pxa_came_workspace_bytes", "pxa_came_flat",
+           "pxa_lcm_step", "pxa_lcm_teacher_target", "pxa_lcm_consistency_loss", "pxa_ema_flat")
 
 _lib = None
 
@@ -198,7 +238,9 @@ def load() -> C.CDLL:
                              ("pxa_ln_prepare", LnPrepareArgs), ("pxa_adamw_flat", AdamWArgs),
                              ("pxa_mlp_fused_bf16", MlpArgs), ("pxa_t5_attn_d64_bf16", T5AttnArgs),
                              ("pxa_sa_solver_step", SaStepArgs), ("pxa_grad_clip_flat", GradClipArgs),
-                             ("pxa_came_flat", CameArgs)):
+                             ("pxa_came_flat", CameArgs), ("pxa_lcm_step", LcmStepArgs),
+                             ("pxa_lcm_teacher_target", LcmTeacherArgs), ("pxa_lcm_consistency_loss", LcmLossArgs),
+                             ("pxa_ema_flat", EmaArgs)):
             fn = getattr(lib, name)
             fn.restype = C.c_int
             fn.argtypes = [C.POINTER(struct), C.c_void_p]
@@ -562,6 +604,107 @@ def sa_solver_step(model_out: torch.Tensor, x: torch.Tensor, x_pred: torch.Tenso
                       p_m1=p_m1, p_noise=p_noise)
     _check(load().pxa_sa_solver_step(C.byref(args), _stream()), "pxa_sa_solver_step")
     return x_pred
+
+
+def _lcm_out(t: torch.Tensor, rows: int, h: int, w: int, what: str) -> None:
+    """A denoiser output an LCM kernel reads: CUDA, fp32 / bf16, (rows, >=4, h, w) with dense (h, w) planes."""
+    if not (t.is_cuda and t.dtype in (torch.float32, torch.bfloat16) and t.dim() == 4):
+        raise PxaError(f"{what}: a 4-D fp32 or bf16 CUDA tensor is required")
+    if t.shape[0] != rows or t.shape[1] < 4 or tuple(t.shape[2:]) != (h, w):
+        raise PxaError(f"{what}: shape {tuple(t.shape)}, expected ({rows}, >=4, {h}, {w})")
+    if not (t.stride(3) == 1 and t.stride(2) == w and t.stride(1) == h * w):
+        raise PxaError(f"{what}: (h, w) planes must be dense")
+
+
+def _lcm_latents(*ts: Optional[torch.Tensor], like: torch.Tensor) -> None:
+    for t in ts:
+        if t is not None and not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.shape == like.shape):
+            raise PxaError(f"latent tensors must be contiguous fp32 CUDA tensors of shape {tuple(like.shape)}")
+
+
+def lcm_step(model_out: torch.Tensor, x: torch.Tensor, noise: Optional[torch.Tensor], denoised: torch.Tensor,
+             x_next: torch.Tensor, *, sqrt_alpha: float, sqrt_beta: float, c_skip: float, c_out: float, c_prev: float,
+             c_noise: float) -> None:
+    """One LCM sampler step (include/pixart_sm100.h: pxa_lcm_step): denoised and x_next written (x_next may be x).
+    model_out: (n, >=4, h, w) fp32 / bf16 (a channel slice is fine); x, noise, denoised, x_next: fp32 (n, 4, h, w)
+    contiguous; noise may be None when c_noise is 0."""
+    if not (x.dim() == 4 and x.shape[1] == 4):
+        raise PxaError("x must be (n, 4, h, w)")
+    n, _, h, w = x.shape
+    _lcm_out(model_out, n, h, w, "model_out")
+    _lcm_latents(x, noise, denoised, x_next, like=x)
+    if noise is None and c_noise != 0.0:
+        raise PxaError("noise is required when c_noise is non-zero")
+    args = LcmStepArgs(model_out=_ptr(model_out), x=_ptr(x), noise=_ptr(noise), denoised=_ptr(denoised), x_next=_ptr(x_next),
+                       out_batch_stride=model_out.stride(0), n=n, hw=h * w, out_dtype=_dt(model_out.dtype),
+                       sqrt_alpha=sqrt_alpha, sqrt_beta=sqrt_beta, c_skip=c_skip, c_out=c_out, c_prev=c_prev, c_noise=c_noise)
+    _check(load().pxa_lcm_step(C.byref(args), _stream()), "pxa_lcm_step")
+
+
+def _lcm_table(index: torch.Tensor, table: torch.Tensor, b: int, dev) -> int:
+    if not (index.is_cuda and index.dtype == torch.int64 and index.is_contiguous() and index.numel() == b and index.device == dev):
+        raise PxaError(f"index must be a contiguous int64 CUDA tensor of {b} elements")
+    row = C.sizeof(LcmRow)
+    if not (table.is_cuda and table.dtype == torch.uint8 and table.numel() % row == 0 and 0 < table.numel() // row <= LCM_MAX_ROWS):
+        raise PxaError("table must be the uint8 device copy of 1..LCM_MAX_ROWS LcmRow entries")
+    return table.numel() // row
+
+
+def lcm_teacher_target(teacher_out: torch.Tensor, x_t: torch.Tensor, index: torch.Tensor, table: torch.Tensor,
+                       x_prev: torch.Tensor, *, w: float) -> torch.Tensor:
+    """Guided DDIM target x_prev (include/pixart_sm100.h: pxa_lcm_teacher_target) from the teacher's output on the batch
+    [cond ; uncond] (2b, >=4, h, w) at x_t (b, 4, h, w); `table` is the device copy of the LcmRow table."""
+    if not (x_t.dim() == 4 and x_t.shape[1] == 4):
+        raise PxaError("x_t must be (b, 4, h, w)")
+    b, _, h, w_ = x_t.shape
+    _lcm_out(teacher_out, 2 * b, h, w_, "teacher_out")
+    _lcm_latents(x_t, x_prev, like=x_t)
+    n_rows = _lcm_table(index, table, b, x_t.device)
+    args = LcmTeacherArgs(teacher_out=_ptr(teacher_out), x_t=_ptr(x_t), index=_ptr(index), table=_ptr(table), x_prev=_ptr(x_prev),
+                          out_batch_stride=teacher_out.stride(0), b=b, hw=h * w_, out_dtype=_dt(teacher_out.dtype),
+                          n_rows=n_rows, w=w)
+    _check(load().pxa_lcm_teacher_target(C.byref(args), _stream()), "pxa_lcm_teacher_target")
+    return x_prev
+
+
+def lcm_consistency_loss(student_out: torch.Tensor, ema_out: torch.Tensor, x_t: torch.Tensor, x_prev: torch.Tensor,
+                         index: torch.Tensor, table: torch.Tensor, d_student_out: torch.Tensor, loss: torch.Tensor,
+                         partials: torch.Tensor, *, loss_type: int = LCM_HUBER, huber_c: float = 1e-3) -> torch.Tensor:
+    """Consistency loss and its gradient (include/pixart_sm100.h: pxa_lcm_consistency_loss).  student_out: the student's
+    fp32 (b, 4 or 8, h, w) output; ema_out: the EMA model's (b, >=4, h, w) output, fp32 or bf16; d_student_out: fp32, the
+    shape of student_out, contiguous; loss: fp32 0-d; partials: fp64 [LCM_LOSS_PARTS] workspace."""
+    if not (x_t.dim() == 4 and x_t.shape[1] == 4):
+        raise PxaError("x_t must be (b, 4, h, w)")
+    b, _, h, w = x_t.shape
+    _lcm_out(student_out, b, h, w, "student_out")
+    _lcm_out(ema_out, b, h, w, "ema_out")
+    if student_out.dtype != torch.float32 or student_out.shape[1] not in (4, 8):
+        raise PxaError("student_out must be the fp32 (b, 4 or 8, h, w) output of the student")
+    _lcm_latents(x_t, x_prev, like=x_t)
+    if not (d_student_out.is_cuda and d_student_out.dtype == torch.float32 and d_student_out.is_contiguous()
+            and d_student_out.shape == student_out.shape):
+        raise PxaError("d_student_out must be a contiguous fp32 CUDA tensor shaped like student_out")
+    if not (loss.is_cuda and loss.dtype == torch.float32 and loss.numel() == 1):
+        raise PxaError("loss must be a one-element fp32 CUDA tensor")
+    if not (partials.is_cuda and partials.dtype == torch.float64 and partials.is_contiguous() and partials.numel() >= LCM_LOSS_PARTS):
+        raise PxaError(f"partials must be a contiguous fp64 CUDA tensor of {LCM_LOSS_PARTS} elements")
+    n_rows = _lcm_table(index, table, b, x_t.device)
+    args = LcmLossArgs(student_out=_ptr(student_out), ema_out=_ptr(ema_out), x_t=_ptr(x_t), x_prev=_ptr(x_prev), index=_ptr(index),
+                       table=_ptr(table), d_student_out=_ptr(d_student_out), loss=_ptr(loss), partials=_ptr(partials),
+                       student_batch_stride=student_out.stride(0), ema_batch_stride=ema_out.stride(0), b=b, hw=h * w,
+                       ema_dtype=_dt(ema_out.dtype), n_rows=n_rows, out_channels=student_out.shape[1], loss_type=loss_type,
+                       huber_c=huber_c)
+    _check(load().pxa_lcm_consistency_loss(C.byref(args), _stream()), "pxa_lcm_consistency_loss")
+    return loss
+
+
+def ema_flat(table: torch.Tensor, *, n_buckets: int, max_n: int, rate: float) -> None:
+    """ema = ema * rate + (1 - rate) * src over every bucket of a device EmaBucket table, with the bf16 shadow written in the
+    same pass (include/pixart_sm100.h: pxa_ema_flat).  The caller keeps the tensors behind the table's pointers alive."""
+    if not (table.is_cuda and table.dtype == torch.uint8 and table.numel() == n_buckets * C.sizeof(EmaBucket)):
+        raise PxaError("table must be the uint8 device copy of n_buckets EmaBucket entries")
+    args = EmaArgs(table=_ptr(table), n_buckets=n_buckets, max_n=max_n, rate=rate)
+    _check(load().pxa_ema_flat(C.byref(args), _stream()), "pxa_ema_flat")
 
 
 # ------------------------------------------------------------------------------------------------- training backward
