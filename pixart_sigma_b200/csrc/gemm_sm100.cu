@@ -115,7 +115,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     EpiConst* consts = reinterpret_cast<EpiConst*>(epi_smem + Cfg::kEpiBufs);
     float2* wg_stats = reinterpret_cast<float2*>(epi_smem + Cfg::kEpiSmem - Cfg::kStatBytes);
     uint8_t* stg = epi_smem + g * Cfg::kAccChunkBytes;                                   // accumulator staging chunk of this warpgroup
-    uint8_t* stile = epi_smem + 2 * Cfg::kAccChunkBytes + (warp - kEpiWarp0) * 4096;     // per-warp transpose tile
+    uint8_t* stile = stg + q * 4096;                                                     // this warp's staging rows
     int stage = 0;
     uint32_t phase = 0;
     int titer = 0;
@@ -218,6 +218,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
             const uint4 u = *reinterpret_cast<const uint4*>(stg + r * 128 + ((c ^ (r & 7)) << 4));
             v[4 * c] = u.x; v[4 * c + 1] = u.y; v[4 * c + 2] = u.z; v[4 * c + 3] = u.w;
           }
+          __syncwarp();                                             // the warp's staging rows are read: they become its stile
           if constexpr (kF32Res) {
             residual_chunk_row_c(v, p, cb, r, cc * 32, m0 + r, n0 + cc * 32, reduce, st);
           } else if constexpr (EPI == PXA_EPI_BIAS_RESIDUAL) {
