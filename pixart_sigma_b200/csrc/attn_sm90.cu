@@ -19,6 +19,7 @@ extern "C" int pxa_flash_attn_d72_bf16(const PxaAttnArgs* args, void* stream) {
   if (a.variant != 0 && (a.variant < 2 || a.variant > 7)) return fail(PXA_ERR_ARG, "variant must be 0 or 2..7");
   if (a.p_precision != 0 && a.p_precision != 1) return fail(PXA_ERR_ARG, "p_precision must be 0 (bf16 P) or 1 (bf16 hi + lo P)");
   if (a.variant == 3 && a.p_precision) return fail(PXA_ERR_ARG, "variant 3 has no p_precision = 1 form");
+  if (!(a.scale >= 0.f)) return fail(PXA_ERR_ARG, "scale must be >= 0");   // the kernel takes the row max on unscaled logits
   FaParams p = {};
   p.out = reinterpret_cast<__nv_bfloat16*>(a.out);
   p.lse = a.lse;
@@ -29,7 +30,21 @@ extern "C" int pxa_flash_attn_d72_bf16(const PxaAttnArgs* args, void* stream) {
   p.reverse_batch = a.reverse_batch ? 1 : 0;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const long long q_rows = (long long)a.B * a.Nq;
-  if (a.p_precision)
-    return launch_flash_fwd<kD, false, true>(a.q, a.k, a.v, q_rows, a.kv_rows, a.q_sn, a.q_sh, a.k_sn, a.k_sh, a.v_sn, a.v_sh, p, s);
-  return launch_flash_fwd<kD, false, false>(a.q, a.k, a.v, q_rows, a.kv_rows, a.q_sn, a.q_sh, a.k_sn, a.k_sh, a.v_sn, a.v_sh, p, s);
+  FaMaps maps;
+  const void* base[3] = {a.q, a.k, a.v};
+  const long long rows[3] = {q_rows, a.kv_rows, a.kv_rows}, sn[3] = {a.q_sn, a.k_sn, a.v_sn}, sh[3] = {a.q_sh, a.k_sh, a.v_sh};
+  CUtensorMap* m[3] = {maps.q, maps.k, maps.v};
+  for (int t = 0; t < 3; ++t) {
+    const int box_rows = t == 0 ? kFaTileQ : kFaBlk;
+    int rc = make_fa_map(&m[t][0], base[t], kD, a.H, rows[t], sn[t], sh[t], 64, box_rows, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (!rc) rc = make_fa_map(&m[t][1], base[t], kD, a.H, rows[t], sn[t], sh[t], 16, box_rows, CU_TENSOR_MAP_SWIZZLE_32B);
+    if (rc) return rc;
+  }
+  auto kernel = a.p_precision ? flash_fwd_d72_kernel<true> : flash_fwd_d72_kernel<false>;
+  PXA_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFaSmem));
+  dim3 grid((a.Nq + kFaTileQ - 1) / kFaTileQ, a.H, a.B);
+  kernel<<<grid, kFaThreads, kFaSmem, s>>>(maps, p);
+  launch_counter()++;
+  PXA_CHECK_CUDA(cudaGetLastError());
+  return PXA_OK;
 }

@@ -178,6 +178,16 @@ template <int kR> PXA_DEVICE void wgmma_fence_regs(float (&d)[kR]) {
 // descriptors (TA / TB = 1: the operand is MN-major); wgmma_rs: A from registers (the mma.sync m16n8k16 A-fragment layout per warp:
 // warp w of the warpgroup holds rows 16 w .. 16 w + 15).  Accumulator layout per thread: d[4 j + 2 h + e] = element
 // (row 16 w + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e).
+template <int TB> PXA_DEVICE void wgmma_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "{%8, %9, %10, %11}, %12, p, 1, 1, %14;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate), "n"(TB));
+}
 template <int TA, int TB> PXA_DEVICE void wgmma_ss_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
@@ -266,7 +276,8 @@ template <int N, int TA, int TB> PXA_DEVICE void wgmma_ss(float (&d)[N / 2], uin
   else { static_assert(N == 128, "unsupported wgmma N"); wgmma_ss_n128<TA, TB>(d, a_desc, b_desc, accumulate); }
 }
 template <int N, int TB> PXA_DEVICE void wgmma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
-  if constexpr (N == 64) wgmma_rs_n64<TB>(d, a, b_desc, accumulate);
+  if constexpr (N == 16) wgmma_rs_n16<TB>(d, a, b_desc, accumulate);
+  else if constexpr (N == 64) wgmma_rs_n64<TB>(d, a, b_desc, accumulate);
   else if constexpr (N == 80) wgmma_rs_n80<TB>(d, a, b_desc, accumulate);
   else if constexpr (N == 96) wgmma_rs_n96<TB>(d, a, b_desc, accumulate);
   else { static_assert(N == 128, "unsupported wgmma N"); wgmma_rs_n128<TB>(d, a, b_desc, accumulate); }
