@@ -566,6 +566,43 @@ typedef struct PxaEmaArgs {
 } PxaEmaArgs;
 int pxa_ema_flat(const PxaEmaArgs* args, void* stream);
 
+/* ------------------------------------------------------------------------------------ DMD distribution-matching loss
+ * The glue of one distribution-matching step (train_scripts/train_pixart_dmd.py:519-561, `use_dm`, `snr_gamma=None`) between
+ * the one-step generator's x0 (`latents`), the frozen real model's CFG batch and the fake model's output, per element:
+ *     a = alphas_cumprod[t[i]],  sa = sqrt(a),  sb = sqrt(1 - a)                  (fp32; t outside [0, n_timesteps): NaN)
+ *     score_real = -(eps_u + cfg (eps_c - eps_u)),  score_fake = -eps_f
+ *     coeff  = (score_fake - score_real) sb / sa,   pred = (noisy + sb score_real) / sa
+ *     weight[i] = 1 / (mean_i |latents - pred| + 1e-5)                            (per sample; the mean from an fp64 sum)
+ *     target = latents - weight coeff,   d = latents - target,   loss = mean(d^2) over b * 4 * hw
+ *     d_gen_out[:, 0:4] = (2 d / (b * 4 * hw)) / gen_sqrt_alpha * (-gen_sqrt_beta)   (dL/deps of x0 = (x - sb_g eps) / sa_g)
+ *     d_gen_out[:, 4:out_channels] = 0 exactly
+ * Every product, sum and division is rounded once, in the reference's fp32 order (the mean over a sample and the loss are
+ * summed in fp64).  Launch 1: PXA_DMD_PARTS CTAs per sample write fp64 partial sums of |latents - pred|; launch 2: each CTA
+ * folds its sample's partials in index order into weight and writes the gradient and fp64 loss partials; launch 3: one CTA
+ * sums the loss partials in index order.  No floating-point atomics: bitwise reproducible, never syncs the host.
+ * real_out: [2b, >=4, hw] with rows 0..b-1 unconditional; fake_out: [b, >=4, hw]; both fp32 or bf16, channel slices fine.
+ * latents, noisy: fp32 [b, 4, hw] contiguous. */
+#define PXA_DMD_PARTS 64
+typedef struct PxaDmdLossArgs {
+  const float* latents;         /* fp32 [b, 4, hw]: the generator's x0                                          */
+  const float* noisy;           /* fp32 [b, 4, hw]: add_noise(latents, noise, t)                                */
+  const int64_t* timesteps;     /* DEVICE [b]                                                                  */
+  const float* alphas_cumprod;  /* DEVICE fp32 [n_timesteps]                                                   */
+  const void* real_out;         /* [2b, >=4, hw], dtype real_dtype, row r at r * real_batch_stride             */
+  const void* fake_out;         /* [b, >=4, hw], dtype fake_dtype, row r at r * fake_batch_stride              */
+  float* d_gen_out;             /* fp32 [b, out_channels, hw] contiguous out                                   */
+  float* loss;                  /* fp32 [1] out                                                                */
+  float* weight;                /* fp32 [b] out                                                                */
+  double* partials;             /* fp64 [2 * b * PXA_DMD_PARTS] workspace                                      */
+  int64_t real_batch_stride, fake_batch_stride;
+  int32_t b, hw, n_timesteps;
+  int32_t out_channels;         /* 4 or 8                                                                      */
+  int32_t real_dtype, fake_dtype;
+  float cfg;                    /* guidance scale of the real model                                            */
+  float gen_sqrt_alpha, gen_sqrt_beta;  /* fp32 sqrt(ac[t_g]), sqrt(1 - ac[t_g]) of the generator's step       */
+} PxaDmdLossArgs;
+int pxa_dmd_loss(const PxaDmdLossArgs* args, void* stream);
+
 /* =============================================================================================== training backward
  * The reference trains through torch autograd (train_scripts/train.py:197 `accelerator.backward(loss)`, per-block
  * activation checkpointing diffusion/model/utils.py:28-45).  The entry points below are the backward twins of the forward

@@ -28,8 +28,8 @@ from . import lib
 from .sampler import _capture, _denoiser_key, _denoiser_params, _step_input
 from .training import IDDPMLoss
 
-__all__ = ["LCMScheduler", "LCMSchedulerOutput", "LCMSampler", "LCMDistiller", "GraphedLCMStep", "boundary_scalings",
-           "distill_table"]
+__all__ = ["LCMScheduler", "LCMSchedulerOutput", "LCMSampler", "LCMDistiller", "GraphedLCMStep", "FlatEMA",
+           "boundary_scalings", "distill_table"]
 
 
 def boundary_scalings(timestep: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -279,13 +279,72 @@ def _inference_copy(model: torch.nn.Module) -> torch.nn.Module:
     return m
 
 
-def _check_ema_forward(ema: torch.nn.Module) -> None:
+def _check_ema_forward(ema: torch.nn.Module, owner: str) -> None:
     """The EMA model's weights are rewritten by a kernel, which does not bump `_version`: the forward modes that keep
     copies derived from the weights and keyed on `_version` (fused LayerNorm-modulate, batched kv_linear) would go stale."""
     from . import model as _m
     if getattr(ema, "fuse_ln_modulate", False) or (_m._KV_BATCH and len(getattr(ema, "blocks", ())) > 1):
-        raise RuntimeError("LCMDistiller: the EMA model cannot use fuse_ln_modulate or PXA_KV_BATCH=1 (their derived weight "
+        raise RuntimeError(f"{owner}: the EMA model cannot use fuse_ln_modulate or PXA_KV_BATCH=1 (their derived weight "
                            "copies are keyed on _version, which pxa_ema_flat does not bump)")
+
+
+class FlatEMA:
+    """An EMA of a model whose parameters a `GradBucketReducer` has flattened: an fp32 master in the reducer's bucket layout
+    and an EMA model (default: a bf16 copy of `model`) whose bucketed parameters are bf16 views of one shadow buffer per
+    bucket.  `update(rate)` is one `pxa_ema_flat` launch, `ema = ema * rate + (1 - rate) * param`, over every bucket; it
+    writes the master and the EMA model's weights.  A given `ema` is initialised from its own values."""
+
+    def __init__(self, model: torch.nn.Module, reducer, ema: Optional[torch.nn.Module] = None, owner: str = "FlatEMA"):
+        self.reducer, self.owner = reducer, owner
+        names = {id(p): n for n, p in model.named_parameters()}
+        given = ema is not None
+        self.ema = ema if given else _inference_copy(model)
+        self.ema.requires_grad_(False)
+        ema_params = dict(self.ema.named_parameters())
+        self.master, self.shadow, self.layout = [], [], []
+        entries = []
+        with torch.no_grad():
+            for b in reducer.buckets:
+                fp = b["flat_param"]
+                master = torch.zeros_like(fp)
+                shadow = torch.zeros(fp.numel(), dtype=torch.bfloat16, device=fp.device)
+                off, layout = 0, []
+                for p in b["params"]:
+                    name, n = names[id(p)], p.numel()
+                    e = ema_params.get(name)
+                    if e is None or e.shape != p.shape:
+                        raise ValueError(f"{owner}: the EMA model has no parameter {name!r} of shape {tuple(p.shape)}")
+                    master[off: off + n].copy_((e if given else p).detach().reshape(-1))
+                    layout.append((name, off, p.shape))
+                    off += n
+                shadow[:off].copy_(master[:off])
+                for name, o, shape in layout:
+                    ema_params[name].data = shadow[o: o + int(np.prod(shape))].view(shape)
+                self.master.append(master)
+                self.shadow.append(shadow)
+                self.layout.append(layout)
+                entries.append(lib.EmaBucket(master=master.data_ptr(), src=fp.data_ptr(), shadow=shadow.data_ptr(), n=off))
+            for e in self.ema.parameters():                   # parameters outside the buckets: plain bf16 copies
+                if e.dtype != torch.bfloat16:
+                    e.data = e.data.to(torch.bfloat16)
+        self._n = [e.n for e in entries]
+        self._table = _upload((lib.EmaBucket * len(entries))(*entries), reducer.buckets[0]["flat_param"].device)
+        _check_ema_forward(self.ema, owner)
+
+    @torch.no_grad()
+    def update(self, rate: float) -> None:
+        """One launch over every bucket; the model's parameters must still be the reducer's flat buckets."""
+        self.reducer.flatten_params()
+        lib.ema_flat(self._table, n_buckets=len(self._n), max_n=max(self._n), rate=rate)
+
+    def state_dict(self) -> Dict[str, torch.Tensor]:
+        """The EMA model's state dict with every bucketed parameter as its fp32 master value; buffers as the EMA model holds
+        them."""
+        sd = {k: v.detach().clone() for k, v in self.ema.state_dict().items()}
+        for master, layout in zip(self.master, self.layout):
+            for name, off, shape in layout:
+                sd[name] = master[off: off + int(np.prod(shape))].view(shape).clone()
+        return sd
 
 
 class _ConsistencyLoss(torch.autograd.Function):
@@ -351,60 +410,24 @@ class LCMDistiller:
         self.uncond = student.y_embedder.y_embedding.detach().clone()     # train_pixart_lcm.py:191 (fixed at start)
         self.teacher = teacher if teacher is not None else _inference_copy(student)
         self.teacher.requires_grad_(False)
-        self._build_ema(ema)
+        self._flat_ema = FlatEMA(student, reducer, ema, owner="LCMDistiller")
 
-    # ---- EMA: fp32 master + bf16 forward weights, both in the reducer's bucket layout
-    def _build_ema(self, ema):
-        names = {id(p): n for n, p in self.student.named_parameters()}
-        given = ema is not None
-        self.ema = ema if given else _inference_copy(self.student)
-        self.ema.requires_grad_(False)
-        ema_params = dict(self.ema.named_parameters())
-        self.master, self.shadow, self.layout = [], [], []
-        entries = []
-        with torch.no_grad():
-            for b in self.reducer.buckets:
-                fp = b["flat_param"]
-                master = torch.zeros_like(fp)
-                shadow = torch.zeros(fp.numel(), dtype=torch.bfloat16, device=fp.device)
-                off, layout = 0, []
-                for p in b["params"]:
-                    name, n = names[id(p)], p.numel()
-                    e = ema_params.get(name)
-                    if e is None or e.shape != p.shape:
-                        raise ValueError(f"LCMDistiller: the EMA model has no parameter {name!r} of shape {tuple(p.shape)}")
-                    master[off: off + n].copy_((e if given else p).detach().reshape(-1))
-                    layout.append((name, off, p.shape))
-                    off += n
-                shadow[:off].copy_(master[:off])
-                for name, o, shape in layout:
-                    ema_params[name].data = shadow[o: o + int(np.prod(shape))].view(shape)
-                self.master.append(master)
-                self.shadow.append(shadow)
-                self.layout.append(layout)
-                entries.append(lib.EmaBucket(master=master.data_ptr(), src=fp.data_ptr(), shadow=shadow.data_ptr(), n=off))
-            for e in self.ema.parameters():                   # parameters outside the buckets: plain bf16 copies
-                if e.dtype != torch.bfloat16:
-                    e.data = e.data.to(torch.bfloat16)
-        self._ema_n = [e.n for e in entries]
-        self._ema_table = _upload((lib.EmaBucket * len(entries))(*entries), self.device)
-        _check_ema_forward(self.ema)
+    # ---- EMA: fp32 master + bf16 forward weights, both in the reducer's bucket layout (FlatEMA)
+    ema = property(lambda self: self._flat_ema.ema)
+    master = property(lambda self: self._flat_ema.master)
+    shadow = property(lambda self: self._flat_ema.shadow)
+    layout = property(lambda self: self._flat_ema.layout)
 
     @torch.no_grad()
     def update_ema(self) -> None:
         """`ema_update(model_ema, model, ema_decay)` (train_pixart_lcm.py:48-53) in one launch: fp32 master and the EMA
         model's bf16 weights.  The student's parameters must still be the reducer's flat buckets."""
-        self.reducer.flatten_params()
-        lib.ema_flat(self._ema_table, n_buckets=len(self._ema_n), max_n=max(self._ema_n), rate=self.ema_decay)
+        self._flat_ema.update(self.ema_decay)
 
     def ema_state_dict(self) -> Dict[str, torch.Tensor]:
         """The EMA model's state dict with every bucketed parameter as its fp32 master value (what `save_checkpoint(model_ema=
         ...)` stores as `state_dict_ema`); buffers as the EMA model holds them."""
-        sd = {k: v.detach().clone() for k, v in self.ema.state_dict().items()}
-        for master, layout in zip(self.master, self.layout):
-            for name, off, shape in layout:
-                sd[name] = master[off: off + int(np.prod(shape))].view(shape).clone()
-        return sd
+        return self._flat_ema.state_dict()
 
     # ---- one distillation step
     def draw(self, latents: torch.Tensor):
@@ -432,7 +455,7 @@ class LCMDistiller:
             out_t = self.teacher(torch.cat([x_t, x_t]), torch.cat([start, start]), torch.cat([y, uncond]), mask=m2, data_info=di2)
             x_prev = torch.empty_like(x_t)
             lib.lcm_teacher_target(_step_input(out_t), x_t, index, self.table, x_prev, w=self.w)
-            _check_ema_forward(self.ema)
+            _check_ema_forward(self.ema, "LCMDistiller")
             out_e = self.ema(x_prev, t, y, mask=mask, data_info=data_info)
         return _ConsistencyLoss.apply(out_s, _step_input(out_e), x_t, x_prev, index, self.table, self.partials, self.loss_type,
                                       self.huber_c)

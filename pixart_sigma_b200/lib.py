@@ -179,6 +179,18 @@ class EmaArgs(C.Structure):
     _fields_ = [("table", C.c_void_p), ("n_buckets", C.c_int32), ("max_n", C.c_int64), ("rate", C.c_double)]
 
 
+DMD_PARTS = 64
+
+
+class DmdLossArgs(C.Structure):
+    _fields_ = [("latents", C.c_void_p), ("noisy", C.c_void_p), ("timesteps", C.c_void_p), ("alphas_cumprod", C.c_void_p),
+                ("real_out", C.c_void_p), ("fake_out", C.c_void_p), ("d_gen_out", C.c_void_p), ("loss", C.c_void_p),
+                ("weight", C.c_void_p), ("partials", C.c_void_p), ("real_batch_stride", C.c_int64),
+                ("fake_batch_stride", C.c_int64), ("b", C.c_int32), ("hw", C.c_int32), ("n_timesteps", C.c_int32),
+                ("out_channels", C.c_int32), ("real_dtype", C.c_int32), ("fake_dtype", C.c_int32), ("cfg", C.c_float),
+                ("gen_sqrt_alpha", C.c_float), ("gen_sqrt_beta", C.c_float)]
+
+
 class GateResidualArgs(C.Structure):
     _fields_ = [("x", C.c_void_p), ("y", C.c_void_p), ("gate", C.c_void_p), ("out", C.c_void_p), ("dgate", C.c_void_p),
                 ("gate_batch_stride", C.c_int64), ("rows_per_batch", C.c_int32), ("M", C.c_int32), ("C", C.c_int32)]
@@ -217,7 +229,8 @@ EXPORTS = ("pxa_transpose_bf16", "pxa_gelu_tanh_bf16", "pxa_gate_residual_fwd", 
            "pxa_ln_prepare", "pxa_layernorm_affine_bf16", "pxa_groupnorm_silu_nhwc_bf16", "pxa_adamw_flat", "pxa_mlp_fused_bf16",
            "pxa_rmsnorm_bf16", "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step",
            "pxa_grad_clip_flat", "pxa_came_workspace_bytes", "pxa_came_flat",
-           "pxa_lcm_step", "pxa_lcm_teacher_target", "pxa_lcm_consistency_loss", "pxa_ema_flat")
+           "pxa_lcm_step", "pxa_lcm_teacher_target", "pxa_lcm_consistency_loss", "pxa_ema_flat",
+           "pxa_dmd_loss")
 
 _lib = None
 
@@ -240,7 +253,7 @@ def load() -> C.CDLL:
                              ("pxa_sa_solver_step", SaStepArgs), ("pxa_grad_clip_flat", GradClipArgs),
                              ("pxa_came_flat", CameArgs), ("pxa_lcm_step", LcmStepArgs),
                              ("pxa_lcm_teacher_target", LcmTeacherArgs), ("pxa_lcm_consistency_loss", LcmLossArgs),
-                             ("pxa_ema_flat", EmaArgs)):
+                             ("pxa_ema_flat", EmaArgs), ("pxa_dmd_loss", DmdLossArgs)):
             fn = getattr(lib, name)
             fn.restype = C.c_int
             fn.argtypes = [C.POINTER(struct), C.c_void_p]
@@ -705,6 +718,46 @@ def ema_flat(table: torch.Tensor, *, n_buckets: int, max_n: int, rate: float) ->
         raise PxaError("table must be the uint8 device copy of n_buckets EmaBucket entries")
     args = EmaArgs(table=_ptr(table), n_buckets=n_buckets, max_n=max_n, rate=rate)
     _check(load().pxa_ema_flat(C.byref(args), _stream()), "pxa_ema_flat")
+
+
+def dmd_loss(latents: torch.Tensor, noisy: torch.Tensor, timesteps: torch.Tensor, alphas_cumprod: torch.Tensor,
+             real_out: torch.Tensor, fake_out: torch.Tensor, d_gen_out: torch.Tensor, loss: torch.Tensor, weight: torch.Tensor,
+             partials: torch.Tensor, *, cfg: float, gen_sqrt_alpha: float, gen_sqrt_beta: float) -> torch.Tensor:
+    """Distribution-matching loss, its per-sample weight and the gradient with respect to the generator's output
+    (include/pixart_sm100.h: pxa_dmd_loss).  latents, noisy: fp32 (b, 4, h, w) contiguous; timesteps: int64 (b,);
+    alphas_cumprod: fp32 (T,); real_out: (2b, >=4, h, w) [uncond ; cond], fake_out: (b, >=4, h, w), fp32 or bf16;
+    d_gen_out: fp32 (b, 4 or 8, h, w) contiguous; loss: fp32 0-d; weight: fp32 (b,); partials: fp64 [2 b DMD_PARTS]."""
+    if not (latents.dim() == 4 and latents.shape[1] == 4):
+        raise PxaError("latents must be (b, 4, h, w)")
+    b, _, h, w = latents.shape
+    _lcm_latents(latents, noisy, like=latents)
+    _lcm_out(real_out, 2 * b, h, w, "real_out")
+    _lcm_out(fake_out, b, h, w, "fake_out")
+    dev = latents.device
+    if not (timesteps.is_cuda and timesteps.dtype == torch.int64 and timesteps.is_contiguous() and timesteps.numel() == b
+            and timesteps.device == dev):
+        raise PxaError(f"timesteps must be a contiguous int64 CUDA tensor of {b} elements")
+    if not (alphas_cumprod.is_cuda and alphas_cumprod.dtype == torch.float32 and alphas_cumprod.dim() == 1
+            and alphas_cumprod.is_contiguous() and alphas_cumprod.numel() > 0):
+        raise PxaError("alphas_cumprod must be a contiguous 1-D fp32 CUDA tensor")
+    if not (d_gen_out.is_cuda and d_gen_out.dtype == torch.float32 and d_gen_out.is_contiguous() and d_gen_out.dim() == 4
+            and d_gen_out.shape[0] == b and d_gen_out.shape[1] in (4, 8) and tuple(d_gen_out.shape[2:]) == (h, w)):
+        raise PxaError(f"d_gen_out must be a contiguous fp32 CUDA tensor of shape ({b}, 4 or 8, {h}, {w})")
+    if not (loss.is_cuda and loss.dtype == torch.float32 and loss.numel() == 1):
+        raise PxaError("loss must be a one-element fp32 CUDA tensor")
+    if not (weight.is_cuda and weight.dtype == torch.float32 and weight.is_contiguous() and weight.numel() == b):
+        raise PxaError(f"weight must be a contiguous fp32 CUDA tensor of {b} elements")
+    if not (partials.is_cuda and partials.dtype == torch.float64 and partials.is_contiguous()
+            and partials.numel() >= 2 * b * DMD_PARTS):
+        raise PxaError(f"partials must be a contiguous fp64 CUDA tensor of {2 * b * DMD_PARTS} elements")
+    args = DmdLossArgs(latents=_ptr(latents), noisy=_ptr(noisy), timesteps=_ptr(timesteps), alphas_cumprod=_ptr(alphas_cumprod),
+                       real_out=_ptr(real_out), fake_out=_ptr(fake_out), d_gen_out=_ptr(d_gen_out), loss=_ptr(loss),
+                       weight=_ptr(weight), partials=_ptr(partials), real_batch_stride=real_out.stride(0),
+                       fake_batch_stride=fake_out.stride(0), b=b, hw=h * w, n_timesteps=alphas_cumprod.numel(),
+                       out_channels=d_gen_out.shape[1], real_dtype=_dt(real_out.dtype), fake_dtype=_dt(fake_out.dtype),
+                       cfg=cfg, gen_sqrt_alpha=gen_sqrt_alpha, gen_sqrt_beta=gen_sqrt_beta)
+    _check(load().pxa_dmd_loss(C.byref(args), _stream()), "pxa_dmd_loss")
+    return loss
 
 
 # ------------------------------------------------------------------------------------------------- training backward
