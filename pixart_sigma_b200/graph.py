@@ -12,6 +12,8 @@ from typing import Dict, Optional, Tuple
 
 import torch
 
+from .lora import require_merged as require_lora_merged
+
 
 class GraphedForward:
     """`method`: 'forward' or 'forward_with_dpmsolver' (the two entry points whose tensor arguments are x, timestep, y, mask;
@@ -39,6 +41,7 @@ class GraphedForward:
     @torch.no_grad()
     def __call__(self, x: torch.Tensor, timestep: torch.Tensor, y: torch.Tensor, mask: Optional[torch.Tensor] = None,
                  data_info=None) -> torch.Tensor:
+        require_lora_merged(self.model)           # a graph captured before an adapter was attached would ignore it
         dev = self._params[0].device
         # The kernels read the parameters in place, but the forward also keeps derived copies (the row-stacked kv_linear weights
         # of model._KvBatch, the fused-LN tables) that a captured graph cannot refresh: an in-place update or a re-assignment of

@@ -1,0 +1,281 @@
+"""LoRA adapters on the native PixArtMS, in peft's directory format, with merged-weight sampling.
+
+A LoRA adapter adds s * B A to a frozen linear weight W [N, K]: A [r, K], B [N, r], s = lora_alpha / r (lora_alpha / sqrt(r)
+with rsLoRA).  This is the configuration of `train_scripts/train_pixart_lora_hf.py`: peft's `LoraConfig(r=rank,
+init_lora_weights="gaussian", target_modules=[...])` with lora_alpha left at peft's default of 8, no dropout, no bias.
+
+The adapters attach to the native modules through `convert.py`'s diffusers name mapping.  A fused native projection carries
+one adapter per diffusers projection: `attn.qkv` (to_q, to_k, to_v) keeps A as [3r, K] and only the three diagonal
+[C, r] blocks of B, as a [3, C, r] parameter; `cross_attn.kv_linear` (to_k, to_v) likewise with 2.  The adapter file keeps
+peft's per-projection tensors.
+
+    load_adapter(model, dir)   read `adapter_config.json` + `adapter_model.safetensors` (what `save_pretrained` writes)
+    save_adapter(model, dir)   write the same files, so that `PeftModel.from_pretrained` accepts the directory
+    merge_lora(model)          W <- round(W + s B A) computed in fp32; every sampler and GraphedForward then runs unchanged
+    unmerge_lora(model)        restore the replaced weights bit for bit
+
+A forward of a model whose adapters are attached but not merged raises instead of silently ignoring them.
+"""
+from __future__ import annotations
+
+import json
+import math
+import os
+from typing import Dict, Iterable, List, Optional, Tuple
+
+import torch
+from torch import nn
+
+from . import convert
+
+# train_pixart_lora_hf.py's target list
+TARGET_MODULES = ("to_q", "to_k", "to_v", "to_out.0", "proj_in", "proj_out", "ff.net.0.proj", "ff.net.2", "proj", "linear",
+                  "linear_1", "linear_2")
+LORA_ALPHA = 8                     # peft's default; the reference script does not set it
+CONFIG_NAME = "adapter_config.json"
+WEIGHTS_NAME = "adapter_model.safetensors"
+_PREFIX = "base_model.model."
+
+_BLOCK_TARGETS = [  # (diffusers module suffix, native module suffix, group, groups)
+    ("attn1.to_q", "attn.qkv", 0, 3), ("attn1.to_k", "attn.qkv", 1, 3), ("attn1.to_v", "attn.qkv", 2, 3),
+    ("attn1.to_out.0", "attn.proj", 0, 1),
+    ("attn2.to_q", "cross_attn.q_linear", 0, 1),
+    ("attn2.to_k", "cross_attn.kv_linear", 0, 2), ("attn2.to_v", "cross_attn.kv_linear", 1, 2),
+    ("attn2.to_out.0", "cross_attn.proj", 0, 1),
+    ("ff.net.0.proj", "mlp.fc1", 0, 1), ("ff.net.2", "mlp.fc2", 0, 1),
+]
+
+
+def adaptable_modules(model: nn.Module) -> List[Tuple[str, str, int, int]]:
+    """Every projection of `model` that a LoRA target can name: (diffusers module name, native module name, group, groups).
+    The projections outside the blocks come first, in the order and with the names of convert.py's key mapping, then the
+    blocks one by one."""
+    out = []
+    pairs = convert._GLOBAL + (convert._MICRO if getattr(model, "micro_conditioning", False) else [])
+    for d, r in pairs:
+        if d.endswith(".weight"):
+            out.append((d[:-len(".weight")], r[:-len(".weight")], 0, 1))
+    for i in range(len(model.blocks)):
+        for d, r, g, n in _BLOCK_TARGETS:
+            out.append((f"transformer_blocks.{i}.{d}", f"blocks.{i}.{r}", g, n))
+    return out
+
+
+def _matches(name: str, targets: Iterable[str]) -> bool:
+    """peft's suffix rule for a list of target names: the module name equals a target or ends with '.' + target."""
+    return any(name == t or name.endswith("." + t) for t in targets)
+
+
+def _scale(r: int, alpha: float, use_rslora: bool) -> float:
+    return alpha / math.sqrt(r) if use_rslora else alpha / r
+
+
+def _check_config(r: int, lora_dropout: float, bias: str, use_dora: bool) -> None:
+    if use_dora:
+        raise NotImplementedError("DoRA adapters are not supported")
+    if lora_dropout:
+        raise NotImplementedError("LoRA dropout is not supported (the reference script uses 0)")
+    if bias != "none":
+        raise NotImplementedError(f"LoRA bias={bias!r} is not supported (only 'none')")
+    if r < 1:
+        raise ValueError(f"LoRA rank must be positive (got {r})")
+
+
+def _plan(model: nn.Module, targets: List[str]) -> Dict[str, List[str]]:
+    """native module name -> the diffusers names of its adapters (one per fused projection), for every projection a target
+    matches.  A fused module must be matched whole."""
+    chosen: Dict[str, list] = {}
+    for dname, nname, g, n in adaptable_modules(model):
+        if _matches(dname, targets):
+            chosen.setdefault(nname, [None] * n)[g] = dname
+    for nname, groups in chosen.items():
+        if any(d is None for d in groups):
+            raise NotImplementedError(f"{nname}: the targets adapt only some of the projections fused in this module "
+                                      f"({[d for d in groups if d]}); adapt all or none")
+    return chosen
+
+
+def _peft_shapes(model: nn.Module, plan: Dict[str, List[str]], r: int) -> Dict[str, Tuple[int, ...]]:
+    """peft's key -> shape for every adapter tensor of `plan`."""
+    mods = dict(model.named_modules())
+    out = {}
+    for nname, groups in plan.items():
+        w = mods[nname].weight
+        n_g = w.shape[0] // len(groups)
+        for dname in groups:
+            out[f"{_PREFIX}{dname}.lora_A.weight"] = (r,) + tuple(w.shape[1:])
+            out[f"{_PREFIX}{dname}.lora_B.weight"] = (n_g, r) + ((1, 1) if w.dim() == 4 else ())
+    return out
+
+
+def inject_lora(model: nn.Module, r: int, use_rslora: bool = False, target_modules: Iterable[str] = TARGET_MODULES,
+                generator: Optional[torch.Generator] = None, *, lora_dropout: float = 0.0, bias: str = "none",
+                use_dora: bool = False, lora_alpha: float = LORA_ALPHA) -> List[str]:
+    """Freeze every base parameter of `model` and attach a fresh adapter to each projection a target matches.  Every check
+    runs before the model is touched: a rejected call leaves it unchanged.
+
+    peft's gaussian init: A ~ N(0, (1/r)^2), B = 0.  A is drawn on the CPU from `generator`, one projection after the other
+    in the order of `adaptable_modules` (the projections outside the blocks, then block by block); peft draws in module
+    registration order, so the distribution matches peft's but the draws for a given seed do not.  A and B are fp32
+    parameters named `lora_A` / `lora_B` on the native module.  Returns the diffusers names of the adapted projections."""
+    _check_config(r, lora_dropout, bias, use_dora)
+    if getattr(model, "_lora", None) is not None:
+        raise RuntimeError("the model already carries a LoRA adapter (one adapter per model)")
+    targets = list(target_modules)
+    plan = _plan(model, targets)
+    for p in model.parameters():
+        p.requires_grad_(False)
+    mods = dict(model.named_modules())
+    names = []
+    for nname, groups in plan.items():
+        mod = mods[nname]
+        w = mod.weight
+        G = len(groups)
+        a_shape = (r,) + tuple(w.shape[1:])
+        A = torch.cat([torch.randn(a_shape, generator=generator) / r for _ in range(G)], 0)
+        mod.lora_A = nn.Parameter(A.to(w.device))
+        mod.lora_B = nn.Parameter(torch.zeros(G, w.shape[0] // G, r, device=w.device))
+        mod.__dict__["_lora_names"] = list(groups)
+        names += groups
+    model.__dict__["_lora"] = {"r": r, "alpha": lora_alpha, "use_rslora": use_rslora, "scale": _scale(r, lora_alpha, use_rslora),
+                               "targets": targets, "merged": False}
+    return names
+
+
+def _adapted(model: nn.Module):
+    for name, mod in model.named_modules():
+        if "_lora_names" in mod.__dict__:
+            yield name, mod
+
+
+def _state(model: nn.Module) -> dict:
+    st = getattr(model, "_lora", None)
+    if st is None:
+        raise RuntimeError("the model carries no LoRA adapter (inject_lora / load_adapter first)")
+    return st
+
+
+def require_merged(model: nn.Module) -> None:
+    """Raise when `model` carries an adapter whose weights are not merged: the native forward would ignore it."""
+    st = model.__dict__.get("_lora")
+    if st is not None and not st["merged"]:
+        raise RuntimeError("PixArtMS: a LoRA adapter is attached but not merged, and the native forward does not apply "
+                           "unmerged adapters; call pixart_sigma_b200.merge_lora(model) first")
+
+
+def adapter_state_dict(model: nn.Module) -> Dict[str, torch.Tensor]:
+    """peft's tensors for the adapter: `base_model.model.<diffusers module>.lora_{A,B}.weight`, fp32, contiguous, on the CPU.
+    Linear: A [r, K], B [N, r]; the conv pos_embed.proj: A [r, 4, 2, 2], B [1152, r, 1, 1]."""
+    r = _state(model)["r"]
+    out = {}
+    for _, mod in _adapted(model):
+        conv = mod.weight.dim() == 4
+        for g, dname in enumerate(mod._lora_names):
+            a = mod.lora_A.detach()[g * r:(g + 1) * r]
+            b = mod.lora_B.detach()[g]
+            if conv:
+                b = b[:, :, None, None]
+            out[f"{_PREFIX}{dname}.lora_A.weight"] = a.float().cpu().contiguous()
+            out[f"{_PREFIX}{dname}.lora_B.weight"] = b.float().cpu().contiguous()
+    return out
+
+
+def adapter_config(model: nn.Module) -> dict:
+    """The `adapter_config.json` peft's `save_pretrained` writes for the reference script's LoraConfig."""
+    st = _state(model)
+    return {
+        "alpha_pattern": {}, "auto_mapping": None, "base_model_name_or_path": None, "bias": "none", "fan_in_fan_out": False,
+        "inference_mode": True, "init_lora_weights": "gaussian", "layer_replication": None, "layers_pattern": None,
+        "layers_to_transform": None, "loftq_config": {}, "lora_alpha": st["alpha"], "lora_dropout": 0.0,
+        "megatron_config": None, "megatron_core": "megatron.core", "modules_to_save": None, "peft_type": "LORA",
+        "r": st["r"], "rank_pattern": {}, "revision": None, "target_modules": sorted(st["targets"]), "task_type": None,
+        "use_dora": False, "use_rslora": st["use_rslora"],
+    }
+
+
+def save_adapter(model: nn.Module, directory: str) -> None:
+    """Write the adapter in peft's directory format (adapter_config.json + adapter_model.safetensors)."""
+    from safetensors.torch import save_file
+    os.makedirs(directory, exist_ok=True)
+    sd = adapter_state_dict(model)
+    with open(os.path.join(directory, CONFIG_NAME), "w") as f:
+        json.dump(adapter_config(model), f, indent=2, sort_keys=True)
+    save_file(sd, os.path.join(directory, WEIGHTS_NAME), metadata={"format": "pt"})
+
+
+def _validate_config(cfg: dict) -> None:
+    if cfg.get("peft_type") != "LORA":
+        raise ValueError(f"not a LoRA adapter: peft_type={cfg.get('peft_type')!r}")
+    for key in ("rank_pattern", "alpha_pattern"):
+        if cfg.get(key):
+            raise NotImplementedError(f"per-module {key} is not supported")
+    if cfg.get("layers_to_transform") is not None or cfg.get("fan_in_fan_out"):
+        raise NotImplementedError("layers_to_transform / fan_in_fan_out are not supported")
+    if cfg.get("modules_to_save"):
+        raise NotImplementedError("modules_to_save is not supported")
+    if not isinstance(cfg.get("target_modules"), list) or not cfg["target_modules"]:
+        raise ValueError("adapter_config.json: target_modules must be a non-empty list of module names")
+    _check_config(int(cfg.get("r", 0)), float(cfg.get("lora_dropout", 0.0)), cfg.get("bias", "none"),
+                  bool(cfg.get("use_dora", False)))
+
+
+def load_adapter(model: nn.Module, directory: str) -> List[str]:
+    """Attach the adapter stored in `directory` (peft's format) to `model`.  The config is validated, and every tensor its
+    `target_modules` call for must be present with peft's shape -- no more, no fewer -- before the model is touched: a
+    rejected file leaves the model unchanged.  The adapter stays unmerged; call merge_lora(model) to sample with it."""
+    from safetensors.torch import load_file
+    with open(os.path.join(directory, CONFIG_NAME)) as f:
+        cfg = json.load(f)
+    _validate_config(cfg)
+    if getattr(model, "_lora", None) is not None:
+        raise RuntimeError("the model already carries a LoRA adapter (one adapter per model)")
+    r = int(cfg["r"])
+    sd = load_file(os.path.join(directory, WEIGHTS_NAME))
+    want = _peft_shapes(model, _plan(model, list(cfg["target_modules"])), r)
+    if set(sd) != set(want):
+        missing, extra = sorted(set(want) - set(sd)), sorted(set(sd) - set(want))
+        raise ValueError(f"adapter tensors do not match the targets: missing {missing[:4]}, unexpected {extra[:4]}")
+    for k, shape in want.items():
+        if tuple(sd[k].shape) != shape or not sd[k].is_floating_point():
+            raise ValueError(f"{k}: {sd[k].dtype} {tuple(sd[k].shape)}, expected a floating-point tensor of shape {shape}")
+    names = inject_lora(model, r, use_rslora=bool(cfg.get("use_rslora", False)), target_modules=cfg["target_modules"],
+                        lora_alpha=float(cfg.get("lora_alpha", LORA_ALPHA)))
+    with torch.no_grad():
+        for _, mod in _adapted(model):
+            for g, dname in enumerate(mod._lora_names):
+                mod.lora_A[g * r:(g + 1) * r].copy_(sd[f"{_PREFIX}{dname}.lora_A.weight"])
+                mod.lora_B[g].copy_(sd[f"{_PREFIX}{dname}.lora_B.weight"].reshape(mod.lora_B.shape[1:]))
+    return names
+
+
+def _delta(mod: nn.Module, r: int, s: float) -> torch.Tensor:
+    """s B A in fp32, shaped like mod.weight (block-diagonal over the fused projections)."""
+    A = mod.lora_A.detach().float().flatten(1)                       # [G r, K]
+    B = mod.lora_B.detach().float()                                  # [G, N/G, r]
+    d = torch.cat([B[g] @ A[g * r:(g + 1) * r] for g in range(B.shape[0])], 0)
+    return (s * d).view(mod.weight.shape)
+
+
+def merge_lora(model: nn.Module) -> None:
+    """W <- W + s B A for every adapted projection: computed in fp32 and rounded once to the parameter's dtype.  The replaced
+    weights are kept (on the host) for unmerge_lora."""
+    st = _state(model)
+    if st["merged"]:
+        raise RuntimeError("the LoRA adapter is already merged")
+    with torch.no_grad():
+        for _, mod in _adapted(model):
+            w = mod.weight
+            mod.__dict__["_lora_saved"] = w.detach().to("cpu", copy=True)
+            w.copy_((w.float() + _delta(mod, st["r"], st["scale"])).to(w.dtype))
+    st["merged"] = True
+
+
+def unmerge_lora(model: nn.Module) -> None:
+    """Restore the weights merge_lora replaced, bit for bit."""
+    st = _state(model)
+    if not st["merged"]:
+        raise RuntimeError("the LoRA adapter is not merged")
+    with torch.no_grad():
+        for _, mod in _adapted(model):
+            mod.weight.copy_(mod.__dict__.pop("_lora_saved"))
+    st["merged"] = False

@@ -22,6 +22,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import lib
+from .lora import require_merged as require_lora_merged
 
 __all__ = ["PixArtMS", "PixArtMSBlock", "PixArtMS_XL_2", "MODELS", "build_model", "install_into_reference"]
 
@@ -649,6 +650,7 @@ class PixArtMS(nn.Module):
     def forward(self, x, timestep, y, mask=None, data_info=None, **kwargs):
         """x (B, 4, H, W) latents, timestep (B,), y (B, 1, L, 4096) T5 features, mask (n, L) | (B,1,1,L) | None
         -> (B, 8, H, W)   (PixArtMS.py:165-211)."""
+        require_lora_merged(self)
         w0 = self.blocks[0].attn.qkv.weight
         if _wants_grad(self, x, y):
             # the kernels fix their own precisions (bf16 operands, fp32 accumulation / statistics / residual stream); an
