@@ -86,7 +86,7 @@ typedef struct PxaGemmArgs {
   int32_t lda, ldw, ldo;
   int32_t epilogue;     /* PXA_EPI_*            */
   int32_t out_dtype;    /* PXA_DTYPE_*          */
-  int32_t block_n;      /* 0 = auto (192 when it divides N, else 128); or 128 / 192 / 256           */
+  int32_t block_n;      /* 0 = auto (192 when it divides N, else 128); or 128 / 192 / 256 (fp32 out: 256 runs as 128) */
   int32_t max_ctas;     /* 0 = one CTA per SM; >0 caps the persistent grid (tests)                  */
   int32_t cta_pair;     /* (ignored, see above; must be 0, 1 or 2) */
   int64_t* debug_trace; /* (ignored) */

@@ -1,14 +1,18 @@
 // pxa_gemm_bf16: out = epilogue(A[M,K] . W[N,K]^T + bias) on wgmma tensor cores (sm_90a).
 //
 // Structure (one persistent CTA per SM, 384 threads = 3 warpgroups):
-//   warp 0       TMA producer: A tile 128x64 and W tile BNx64 (bf16, 128B-swizzled) into a kStages-deep smem ring
+//   warp 0       TMA producer: A tile 128x64 and W tile BNx64 (bf16, 128B-swizzled) into a kStages-deep smem ring, and the
+//                tile's epilogue operand (fp32 / bf16 residual, bf16 pre-activation) into the output tile in smem
 //                (the rest of its warpgroup gives its registers away with setmaxnreg and idles)
 //   warps 4-11   two consumer warpgroups.  Warpgroup g owns the 128 x BN/2 half [g BN/2, (g+1) BN/2) of the tile: per K-block
 //                it issues 2 (64-row halves) x 4 (K steps) wgmma.mma_async m64 x BN/2 x 16 with both operands read from the
-//                ring through shared-memory descriptors, fp32 accumulators in registers (BN/2 per thread).  While one
-//                warpgroup waits for its group or runs its epilogue the other one keeps the tensor pipe busy.
-//                Epilogue: 32-column accumulator chunks go through a swizzled smem staging buffer into the row-per-thread
-//                layout (thread = row, 32 consecutive columns) -> bias / GELU / gate*x + residual -> global.
+//                ring through shared-memory descriptors, fp32 accumulators in registers (BN/2 per thread).
+//                Epilogue: bias / GELU / gate * x + residual / LayerNorm-modulate are applied to the accumulator fragments,
+//                the results are written into the warpgroup's half of the swizzled output tile (over the operand) and one
+//                thread issues TMA stores of its 128 x 32 slabs; the warpgroup goes on to the next tile's MMAs while the stores
+//                drain.  Before the output tile is written again, the storing thread waits for the stores' smem reads
+//                (cp.async.bulk.wait_group.read), part way into the next main loop, and then lets the producer load the
+//                next operand into it.
 // Tiles are visited n-fastest so the CTAs running concurrently share the same few A row-blocks through L2 and the
 // whole weight matrix stays L2-resident.
 //
@@ -17,27 +21,46 @@
 
 namespace pxa {
 
+// K-block of a tile (counted from the tile's first) after which the consumers release the output tile of the previous tile:
+// late enough for its stores to have drained, early enough for the next operand to arrive before the tile's epilogue.
+PXA_DEVICE int release_kb(int nk) {
+  const int q = nk / 4 > 1 ? nk / 4 : 1;
+  return q < nk - 1 ? q : nk - 1;
+}
+
 // ------------------------------------------------------------------------------------------------- kernel
 // kMn: both operands are given MN-major -- A as [K, M] (M contiguous), W as [K, N] (N contiguous) -- the layout of the
 // weight-gradient product dW[N, K] = dY[M, N]^T X[M, K], whose contraction runs over the token dimension.  Each K-block
 // is staged as 64-wide swizzle atoms of 64 k-rows (two for the 128 rows of A, BN / 64 for W) and consumed through
 // MN-major descriptors (atoms LBO apart, 16 k-rows = 2048 B per K-step).  With p.k_splits > 1 the K range is split
-// across tiles (split-K); legal only with the reduce-add form of the fp32 residual epilogue, which makes the partial sums add
-// up in L2.
+// across tiles (split-K); legal only with the reduce-add form of the fp32 residual epilogue: the output tile is added into
+// `out` by TMA reductions, so that the partial sums add up in L2.
+//
+// tmap_out / tmap_res: `out` and the epilogue operand as 3-D tensors (column, x, line) with 32 x 128 x 1 boxes.  x runs over
+// the GEMM rows (one line), except for a convolution over a virtual width, where it runs over the W real pixels of an image
+// line: the stores drop the columns x >= W and the rows >= M.
 template <int BN, int EPI, typename OutT, bool kConv = false, bool kMn = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w, const GemmParams p) {
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
+                 const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_res, const GemmParams p) {
   constexpr bool kF32Res = (EPI == PXA_EPI_BIAS_RESIDUAL) && sizeof(OutT) == 4;
-  using Cfg = GemmCfg<BN>;
+  constexpr bool kRes = EPI == PXA_EPI_BIAS_RESIDUAL;
+  constexpr bool kLn = (EPI == PXA_EPI_LN_BIAS || EPI == PXA_EPI_LN_BIAS_GELU);
+  using Cfg = GemmCfg<BN, OutT>;
   constexpr int kStages = Cfg::kStages;
   constexpr int NW = BN / 2;                       // columns per consumer warpgroup
+  constexpr int kSlabs = NW / 32;                  // output slabs per consumer warpgroup
   static_assert(!kMn || NW % 64 == 0, "MN-major W is staged in 64-column atoms");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* epi_smem = smem + kStages * Cfg::kStage;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(epi_smem + Cfg::kEpiSmem);
+  uint8_t* otile = smem + kStages * Cfg::kStage;                                  // output tile: slab cs at cs * kSlabBytes
+  EpiConst<BN>* consts = reinterpret_cast<EpiConst<BN>*>(otile + Cfg::kEpiTile);
+  float2* rowbuf = reinterpret_cast<float2*>(otile + Cfg::kEpiTile + Cfg::kConstBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(otile + Cfg::kEpiSmem);
   uint64_t* full_bar = bars;                    // [kStages]  TMA -> consumers
   uint64_t* empty_bar = bars + kStages;         // [kStages]  consumers -> TMA (one arrival per consumer warp)
+  uint64_t* opnd_full = bars + 2 * kStages;     // the tile's epilogue operand has landed in the output tile
+  uint64_t* opnd_empty = opnd_full + 1;         // the previous tile's stores have read the output tile (one arrival per warpgroup)
 
   const int warp = warp_idx_sync();
   const int lane = threadIdx.x & 31;
@@ -45,10 +68,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_w);
+    prefetch_tmap(&tmap_out);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], kNumEpiThreads / 32);
     }
+    mbar_init(opnd_full, 1);
+    mbar_init(opnd_empty, 2);
     fence_mbar_init();
   }
   __syncthreads();
@@ -62,18 +88,31 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   auto kb_hi = [&](int tile) { return (int)((long long)(tile / mn_tiles + 1) * num_kb / p.k_splits); };
   auto tile_m0 = [&](int tile) { return ((tile % mn_tiles) / p.num_n_tiles) * kBM; };
   auto tile_n0 = [&](int tile) { return ((tile % mn_tiles) % p.num_n_tiles) * BN; };
+  // (x, line) of the tile's first output row in tmap_out / tmap_res
+  auto out_xy = [&](int m0) {
+    if (kConv && p.conv_Wp != p.conv_W) return make_int2(m0 % p.conv_Wp, m0 / p.conv_Wp);
+    return make_int2(m0, 0);
+  };
+  // in-place split-K accumulation: partial sums are added into `out` (no residual read)
+  const bool reduce = kF32Res && p.k_splits > 1;
+  // the epilogue reads a [M, N] operand laid out like `out`: the residual, or the pre-activation of EPI_MUL_DGELU
+  const bool has_opnd = (kRes && !reduce) || EPI == PXA_EPI_MUL_DGELU;
 
   if (warp < kEpiWarp0) {
     // ================================================================ TMA producer
     reg_dealloc<40>();
     if (warp == 0 && elect_one()) {
+      if (has_opnd) prefetch_tmap(&tmap_res);
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+      int titer = 0;
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++titer) {
         const int tile = eff(t);
         const int m0 = tile_m0(tile);
         const int n0 = tile_n0(tile);
-        for (int kb = kb_lo(tile); kb < kb_hi(tile); ++kb) {
+        const int kb0 = kb_lo(tile), kb1 = kb_hi(tile);
+        const int rel = release_kb(kb1 - kb0);
+        for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * Cfg::kStage;
           uint8_t* sb = sa + Cfg::kStageA;
@@ -83,39 +122,42 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
             for (int i = 0; i < kBM / 64; ++i) tma_load_2d(sa + i * 8192, &tmap_a, &full_bar[stage], m0 + 64 * i, kb * kBK, kEvictNormal);
 #pragma unroll
             for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, &tmap_w, &full_bar[stage], n0 + 64 * j, kb * kBK, kEvictNormal);
-            if (++stage == kStages) { stage = 0; phase ^= 1; }
-            continue;
-          }
-          if constexpr (kConv) {
-            // implicit GEMM: K-block kb = (tap, 64-channel slice); the A tile is the tile's pixel block shifted by the
-            // tap offset -- zero padding comes for free from TMA out-of-bounds fill on the W / H dimensions
-            const int tap = kb / p.conv_cin_blocks;
-            const int c0 = (kb - tap * p.conv_cin_blocks) * kBK;
-            const int pix = m0;                                     // first pixel of the tile in (b, y, x) order of the virtual image
-            const int x0 = pix % p.conv_Wp;
-            const int y0 = (pix / p.conv_Wp) % p.conv_H;
-            const int b0 = pix / (p.conv_Wp * p.conv_H);
-            tma_load_4d(sa, &tmap_a, &full_bar[stage], c0, x0 + tap % 3 - 1, y0 + tap / 3 - 1, b0, kEvictNormal);
           } else {
-            tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * kBK, m0, kEvictNormal);
+            if constexpr (kConv) {
+              // implicit GEMM: K-block kb = (tap, 64-channel slice); the A tile is the tile's pixel block shifted by the
+              // tap offset -- zero padding comes for free from TMA out-of-bounds fill on the W / H dimensions
+              const int tap = kb / p.conv_cin_blocks;
+              const int c0 = (kb - tap * p.conv_cin_blocks) * kBK;
+              const int pix = m0;                                     // first pixel of the tile in (b, y, x) order of the virtual image
+              const int x0 = pix % p.conv_Wp;
+              const int y0 = (pix / p.conv_Wp) % p.conv_H;
+              const int b0 = pix / (p.conv_Wp * p.conv_H);
+              tma_load_4d(sa, &tmap_a, &full_bar[stage], c0, x0 + tap % 3 - 1, y0 + tap / 3 - 1, b0, kEvictNormal);
+            } else {
+              tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * kBK, m0, kEvictNormal);
+            }
+            tma_load_2d(sb, &tmap_w, &full_bar[stage], kb * kBK, n0, kEvictLast);
           }
-          tma_load_2d(sb, &tmap_w, &full_bar[stage], kb * kBK, n0, kEvictLast);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
+          if (has_opnd && kb - kb0 == rel) {
+            // the consumers release the output tile at this K-block of the tile (see release_kb)
+            mbar_wait(opnd_empty, titer & 1);
+            const int slabs = (p.N - n0 + 31) / 32 < BN / 32 ? (p.N - n0 + 31) / 32 : BN / 32;
+            mbar_arrive_expect_tx(opnd_full, slabs * Cfg::kSlabBytes);
+            const int2 xy = out_xy(m0);
+            for (int cs = 0; cs < slabs; ++cs)
+              tma_load_3d(otile + cs * Cfg::kSlabBytes, &tmap_res, opnd_full, n0 + 32 * cs, xy.x, xy.y, kEvictNormal);
+          }
         }
       }
     }
   } else {
     // ================================================================ consumers: wgmma main loop + epilogue
     reg_alloc<232>();
-    constexpr bool kLn = (EPI == PXA_EPI_LN_BIAS || EPI == PXA_EPI_LN_BIAS_GELU);
     const int g = (warp - kEpiWarp0) >> 2;          // consumer warpgroup = column half of the tile
-    const int q = warp & 3;                         // this warp's 32-row quarter of the tile in the epilogue
+    const int q = warp & 3;                         // this warp's 16-row slice of each 64-row half of the tile
     const int tid = threadIdx.x - kEpiWarp0 * 32;   // 0..255
-    const int r = q * 32 + lane;                    // row of the 128-row tile owned by this thread in the epilogue
-    EpiConst* consts = reinterpret_cast<EpiConst*>(epi_smem + Cfg::kEpiBufs);
-    float2* wg_stats = reinterpret_cast<float2*>(epi_smem + Cfg::kEpiSmem - Cfg::kStatBytes);
-    uint8_t* stg = epi_smem + g * Cfg::kAccChunkBytes;                                   // accumulator staging chunk of this warpgroup
-    uint8_t* stile = stg + q * 4096;                                                     // this warp's staging rows
+    const bool storer = (tid & 127) == 0;           // issues and waits for this warpgroup's TMA stores
     int stage = 0;
     uint32_t phase = 0;
     int titer = 0;
@@ -124,20 +166,18 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if ((int)blockIdx.x < num_tiles) {
       const int ft = eff(blockIdx.x);
       load_epi_consts<BN, kLn>(er, p, tid, tile_m0(ft), tile_n0(ft));
-      if constexpr (kLn) load_ln_stats(sr, p, tile_m0(ft) + r);
+      if constexpr (kLn) if (g == 0) load_ln_stats(sr, p, tile_m0(ft) + tid);
     }
-    // in-place split-K accumulation: partial sums are added into `out` (no residual read)
-    const bool reduce = kF32Res && p.k_splits > 1;
     float acc[2][NW / 2];
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++titer) {
       const int tile = eff(t);
       const int m0 = tile_m0(tile);
       const int n0 = tile_n0(tile);
-      const int nch = chunks_of_tile<BN>(p, n0);
       // ---- main loop
       // One wgmma group stays in flight: the group of K-block kb is committed before the group of kb - 1 is waited for, and a
       // stage goes back to the producer once the group that read it has completed.
       const int kb0 = kb_lo(tile), kb1 = kb_hi(tile);
+      const int rel = release_kb(kb1 - kb0);
       int prev_stage = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
@@ -163,91 +203,175 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);   // this warp has finished reading that stage
         prev_stage = stage;
         if (++stage == kStages) { stage = 0; phase ^= 1; }
+        if (kb - kb0 == rel && storer) {            // the previous tile's stores have read this warpgroup's slabs
+          tma_store_wait_read<0>();
+          if (has_opnd) mbar_arrive(opnd_empty);
+        }
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc[0]);
       wgmma_fence_regs(acc[1]);
       if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
       // ---- epilogue
-      EpiConst* cb = consts + (titer & 1);
+      EpiConst<BN>* cb = consts + (titer & 1);
+      float2* lnc = rowbuf + (titer & 1) * kBM;                    // LN consumer: (rstd, -rstd * mean) of each tile row
       store_epi_consts<BN>(cb, er, tid);
-      [[maybe_unused]] float2 ln = make_float2(1.f, 0.f);
-      if constexpr (kLn) ln = ln_row_coeffs(p, sr);
+      if constexpr (kLn) if (g == 0) lnc[tid] = ln_row_coeffs(p, sr);
       named_bar_sync(2, kNumEpiThreads);
-      if (t + (int)gridDim.x < num_tiles) {                          // next tile's loads: in flight during this tile's chunks
+      if (has_opnd) mbar_wait(opnd_full, titer & 1);
+      const int row_split = cb->row_split;
+      // samples shorter than a tile (rows_per_batch < 128, tiny images): a tile may span more than two samples, so the gate row
+      // is looked up per row in global memory instead of the two staged rows
+      const bool per_row_gate = kRes && p.gate != nullptr && p.rows_per_batch < kBM;
+      __nv_bfloat16* aux = p.out_aux;
+      [[maybe_unused]] float2 st[2][2] = {};                        // (sum, sum of squares) of each of this thread's rows
+      // fragment (i, j, h) of this thread: tile row 64 i + 16 q + lane / 4 + 8 h, warpgroup columns 8 j + 2 (lane % 4) + {0, 1}
+#pragma unroll
+      for (int s = 0; s < kSlabs; ++s) {
+        const int cs = g * kSlabs + s;                              // slab of the tile (warpgroup-uniform)
+        if (n0 + 32 * cs >= p.N) continue;
+        uint8_t* slab = otile + cs * Cfg::kSlabBytes;
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = 64 * i + 16 * q + (lane >> 2) + 8 * h;
+            const int grow = m0 + row;
+            const bool second = row >= row_split;
+            [[maybe_unused]] float2 ln = make_float2(1.f, 0.f);
+            if constexpr (kLn) ln = lnc[row];
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int c = 8 * jj + 2 * (lane & 3);                // column in the slab
+              const int tc = 32 * cs + c;                           // column in the tile
+              const int gcol = n0 + tc;
+              const float a0 = acc[i][4 * (4 * s + jj) + 2 * h], a1 = acc[i][4 * (4 * s + jj) + 2 * h + 1];
+              uint8_t* e = slab + slab_offset<OutT>(row, c);
+              const bool aux_ok = aux != nullptr && grow < p.M && gcol < p.N;
+              const size_t off = (size_t)grow * p.ldo + gcol;
+              if constexpr (kRes) {
+                // out = residual + gate * (acc + bias); aux = bf16 of out or of the branch output acc + bias (aux_branch),
+                // times aux_scale of the row's sample when given
+                const float2 b = *reinterpret_cast<const float2*>(cb->bias + tc);
+                float2 gt = *reinterpret_cast<const float2*>((second ? cb->gate1 : cb->gate0) + tc);
+                if (per_row_gate)
+                  gt = (grow < p.M && gcol < p.N)
+                           ? __ldg(reinterpret_cast<const float2*>(p.gate + (size_t)((p.row_base + grow) / p.rows_per_batch) *
+                                                                                 p.gate_batch_stride + gcol))
+                           : make_float2(1.f, 1.f);
+                float2 r = make_float2(0.f, 0.f);
+                if constexpr (sizeof(OutT) == 4) {
+                  if (!reduce) r = *reinterpret_cast<const float2*>(e);
+                } else {
+                  const uint32_t u = *reinterpret_cast<const uint32_t*>(e);
+                  r = make_float2(bf16_lo(u), bf16_hi(u));
+                }
+                const float2 yb = make_float2(a0 + b.x, a1 + b.y);   // the branch output
+                const float2 o = make_float2(fmaf(gt.x, yb.x, r.x), fmaf(gt.y, yb.y, r.y));
+                if constexpr (sizeof(OutT) == 4) {
+                  *reinterpret_cast<float2*>(e) = o;
+                  if (gcol < p.N) {
+                    st[i][h].x += o.x + o.y;
+                    st[i][h].y = fmaf(o.x, o.x, fmaf(o.y, o.y, st[i][h].y));
+                  }
+                } else {
+                  *reinterpret_cast<uint32_t*>(e) = pack_bf16x2(o.x, o.y);
+                }
+                if (aux_ok) {
+                  float2 ax = p.aux_branch ? yb : o;
+                  if (kF32Res && p.aux_scale != nullptr) {
+                    const float2 sc = *reinterpret_cast<const float2*>((second ? cb->ex1 : cb->ex0) + tc);
+                    ax = make_float2(ax.x * sc.x, ax.y * sc.y);
+                  }
+                  *reinterpret_cast<uint32_t*>(aux + off) = pack_bf16x2(ax.x, ax.y);
+                }
+              } else {
+                float x0, x1;
+                if constexpr (kLn) {   // out = [gelu](rstd * (acc - mu * u) + v), u / v of the row's sample
+                  const float2 v = *reinterpret_cast<const float2*>((second ? cb->gate0 : cb->bias) + tc);
+                  const float2 u = *reinterpret_cast<const float2*>((second ? cb->ex1 : cb->ex0) + tc);
+                  x0 = fmaf(ln.x, a0, fmaf(ln.y, u.x, v.x));
+                  x1 = fmaf(ln.x, a1, fmaf(ln.y, u.y, v.y));
+                } else {
+                  const float2 b = *reinterpret_cast<const float2*>(cb->bias + tc);
+                  x0 = a0 + b.x;
+                  x1 = a1 + b.y;
+                }
+                if constexpr (EPI == PXA_EPI_BIAS_GELU_AUX) {       // aux = the pre-activation the GELU backward needs
+                  if (aux_ok) *reinterpret_cast<uint32_t*>(aux + off) = pack_bf16x2(x0, x1);
+                }
+                if constexpr (EPI == PXA_EPI_BIAS_GELU || EPI == PXA_EPI_BIAS_GELU_AUX || EPI == PXA_EPI_LN_BIAS_GELU) {
+                  x0 = gelu_tanh(x0);
+                  x1 = gelu_tanh(x1);
+                }
+                if constexpr (EPI == PXA_EPI_MUL_DGELU) {           // out = acc * gelu'(pre), pre over which out is written
+                  const uint32_t w = *reinterpret_cast<const uint32_t*>(e);
+                  x0 *= gelu_tanh_grad(bf16_lo(w));
+                  x1 *= gelu_tanh_grad(bf16_hi(w));
+                }
+                *reinterpret_cast<uint32_t*>(e) = pack_bf16x2(x0, x1);
+              }
+            }
+          }
+      }
+      if (t + (int)gridDim.x < num_tiles) {                          // next tile's loads: in flight during the next main loop
         const int nt_ = eff(t + gridDim.x);
         load_epi_consts<BN, kLn>(er, p, tid, tile_m0(nt_), tile_n0(nt_));
-        if constexpr (kLn) load_ln_stats(sr, p, tile_m0(nt_) + r);
+        if constexpr (kLn) if (g == 0) load_ln_stats(sr, p, tile_m0(nt_) + tid);
       }
-      [[maybe_unused]] const bool second = r >= cb->row_split;
-      // this warp's 32 output rows: GEMM rows m0 + 32 q ..; a convolution over a virtual width (conv_Wp > W: one image line per
-      // tile) stores pixel x of line (b, y) at row (b H + y) W + x and drops the columns x >= W
-      int row0 = m0 + q * 32;
-      [[maybe_unused]] int m_lim = -1;
-      if constexpr (kConv) {
-        if (p.conv_Wp != p.conv_W) {
-          const int xs = m0 % p.conv_Wp + q * 32;
-          const int left = p.conv_W - xs;
-          row0 = (m0 / p.conv_Wp) * p.conv_W + xs;
-          m_lim = row0 + (left < 0 ? 0 : (left > 32 ? 32 : left));
+      // the warpgroup's slabs are written: one thread hands them to the TMA engine
+      fence_proxy_async_smem();
+      named_bar_sync(4 + g, 128);
+      if (storer) {
+        const int2 xy = out_xy(m0);
+#pragma unroll
+        for (int s = 0; s < kSlabs; ++s) {
+          const int cs = g * kSlabs + s;
+          if (n0 + 32 * cs >= p.N) continue;
+          if (kF32Res && reduce) tma_reduce_add_3d(&tmap_out, otile + cs * Cfg::kSlabBytes, n0 + 32 * cs, xy.x, xy.y);
+          else tma_store_3d(&tmap_out, otile + cs * Cfg::kSlabBytes, n0 + 32 * cs, xy.x, xy.y);
         }
-      }
-      float2 st = make_float2(0.f, 0.f);                            // this row's (sum, sum of squares) over this warpgroup's chunks
-#pragma unroll
-      for (int lc = 0; lc < NW / 32; ++lc) {
-        const int cc = g * (NW / 32) + lc;                          // chunk of the tile (warpgroup-uniform)
-        if (cc < nch) {
-          // fragments -> staging: element (row, col) of the 128 x 32 chunk at row * 128 B + (((col / 4) ^ (row & 7)) * 16) B
-          named_bar_sync(4 + g, 128);                               // the previous chunk has been read
-#pragma unroll
-          for (int i = 0; i < 2; ++i)
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj)
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const int row = 64 * i + 16 * q + (lane >> 2) + 8 * h;
-                const int col = 8 * jj + 2 * (lane & 3);
-                const int j = 4 * lc + jj;
-                *reinterpret_cast<float2*>(stg + row * 128 + (((col >> 2) ^ (row & 7)) << 4) + (col & 3) * 4) =
-                    make_float2(acc[i][4 * j + 2 * h], acc[i][4 * j + 2 * h + 1]);
-              }
-          named_bar_sync(4 + g, 128);
-          uint32_t v[32];
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const uint4 u = *reinterpret_cast<const uint4*>(stg + r * 128 + ((c ^ (r & 7)) << 4));
-            v[4 * c] = u.x; v[4 * c + 1] = u.y; v[4 * c + 2] = u.z; v[4 * c + 3] = u.w;
-          }
-          __syncwarp();                                             // the warp's staging rows are read: they become its stile
-          if constexpr (kF32Res) {
-            residual_chunk_row_c(v, p, cb, r, cc * 32, m0 + r, n0 + cc * 32, reduce, st);
-          } else if constexpr (EPI == PXA_EPI_BIAS_RESIDUAL) {
-            ResFrag res;                                            // bf16 residual stream (VAE convolutions)
-            load_residual_frag<OutT>(res, p, lane, row0, n0 + cc * 32, m_lim);
-            epilogue_chunk_residual<OutT>(v, res, p, stile, lane, row0, n0 + cc * 32, m_lim);
-          } else if constexpr (kLn) {
-            epilogue_chunk_bf16_c<EPI>(v, p, cb, stile, lane, row0, n0 + cc * 32, cc * 32, ln, second);
-          } else {
-            epilogue_chunk_bf16_c<EPI>(v, p, cb, stile, lane, row0, n0 + cc * 32, cc * 32, make_float2(1.f, 0.f), false, m_lim);
-          }
-        }
+        tma_store_commit();
       }
       if constexpr (kF32Res) {
         if (p.row_stats_out != nullptr) {       // partial LayerNorm statistics of this row: part = n tile (both warpgroups' halves)
-          if (g == 1) wg_stats[r] = st;
+          float2* wg_stats = rowbuf;
+#pragma unroll
+          for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int d = 1; d < 4; d <<= 1) {
+                st[i][h].x += __shfl_xor_sync(0xffffffffu, st[i][h].x, d);
+                st[i][h].y += __shfl_xor_sync(0xffffffffu, st[i][h].y, d);
+              }
+          const bool quad_lead = (lane & 3) == 0;
+          if (g == 1 && quad_lead)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) wg_stats[64 * i + 16 * q + (lane >> 2) + 8 * h] = st[i][h];
           named_bar_sync(3, kNumEpiThreads);
-          if (g == 0 && m0 + r < p.M) {
+          if (g == 0 && quad_lead) {
             const int nt = (tile % mn_tiles) % p.num_n_tiles;
-            const float2 o = wg_stats[r];
-            float2* sp = reinterpret_cast<float2*>(p.row_stats_out) + (size_t)(m0 + r) * PXA_LN_STAT_PARTS;
-            sp[nt] = make_float2(st.x + o.x, st.y + o.y);
-            if (nt == p.num_n_tiles - 1)
-              for (int i = p.num_n_tiles; i < PXA_LN_STAT_PARTS; ++i) sp[i] = make_float2(0.f, 0.f);
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int row = 64 * i + 16 * q + (lane >> 2) + 8 * h;
+                if (m0 + row >= p.M) continue;
+                const float2 o = wg_stats[row];
+                float2* sp = reinterpret_cast<float2*>(p.row_stats_out) + (size_t)(m0 + row) * PXA_LN_STAT_PARTS;
+                sp[nt] = make_float2(st[i][h].x + o.x, st[i][h].y + o.y);
+                if (nt == p.num_n_tiles - 1)
+                  for (int k = p.num_n_tiles; k < PXA_LN_STAT_PARTS; ++k) sp[k] = make_float2(0.f, 0.f);
+              }
           }
           named_bar_sync(3, kNumEpiThreads);
         }
       }
     }
+    if (storer) tma_store_wait_all<0>();
   }
 }
 
@@ -297,7 +421,27 @@ static int launch_gemm(const GemmCall& a, cudaStream_t stream, const ConvGeom* c
     int rc = make_tmap_bf16(&tw, a.w, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  using Cfg = GemmCfg<BN>;
+  // out and the epilogue operand (same layout) as (column, x, line): x over the GEMM rows, or over the W pixels of an image line
+  // for a convolution over a virtual width (its columns x >= W are then clipped by the stores)
+  CUtensorMap to, tr;
+  {
+    constexpr uint64_t es = sizeof(OutT);
+    const bool lines = kConv && cg->Wp != cg->W;
+    const uint64_t X = lines ? (uint64_t)cg->W : (uint64_t)a.M;
+    uint64_t dims[3] = {(uint64_t)a.N, X, lines ? (uint64_t)cg->B * cg->H : 1ull};
+    uint64_t str[2] = {(uint64_t)a.ldo * es, X * a.ldo * es};
+    uint32_t box[3] = {32, kBM, 1};
+    const CUtensorMapDataType dt = es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    const CUtensorMapSwizzle swz = es == 4 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+    int rc = make_tmap(&to, dt, a.out, 3, dims, str, box, swz);
+    if (rc) return rc;
+    tr = to;
+    if (a.residual != nullptr) {
+      rc = make_tmap(&tr, dt, a.residual, 3, dims, str, box, swz);
+      if (rc) return rc;
+    }
+  }
+  using Cfg = GemmCfg<BN, OutT>;
   GemmParams p = {};
   p.bias = reinterpret_cast<const __nv_bfloat16*>(a.bias);
   p.out = a.out;
@@ -325,7 +469,7 @@ static int launch_gemm(const GemmCall& a, cudaStream_t stream, const ConvGeom* c
   if (a.max_ctas > 0 && a.max_ctas < grid) grid = a.max_ctas;
   const int tiles = p.num_m_tiles * p.num_n_tiles * p.k_splits;
   if (tiles < grid) grid = tiles;
-  kern<<<grid, kGemmThreads, Cfg::kSmem, stream>>>(ta, tw, p);
+  kern<<<grid, kGemmThreads, Cfg::kSmem, stream>>>(ta, tw, to, tr, p);
   launch_counter()++;
   PXA_CHECK_CUDA(cudaGetLastError());
   return PXA_OK;
@@ -350,7 +494,7 @@ static int dispatch_epi(const GemmCall& a, cudaStream_t s) {
       return launch_gemm<BN, PXA_EPI_LN_BIAS_GELU, __nv_bfloat16>(a, s);
     case PXA_EPI_BIAS_RESIDUAL:
       if (a.residual == nullptr) return fail(PXA_ERR_ARG, "EPI_BIAS_RESIDUAL needs residual");
-      if (a.out_dtype == PXA_DTYPE_F32) return launch_gemm<BN, PXA_EPI_BIAS_RESIDUAL, float>(a, s);
+      if (a.out_dtype == PXA_DTYPE_F32) return launch_gemm<BN == 256 ? 128 : BN, PXA_EPI_BIAS_RESIDUAL, float>(a, s);
       return launch_gemm<BN, PXA_EPI_BIAS_RESIDUAL, __nv_bfloat16>(a, s);
     default:
       return fail(PXA_ERR_ARG, "unknown epilogue %d", a.epilogue);
@@ -457,7 +601,7 @@ int gemm_bf16_rows(const PxaGemmArgs* args, int row_base, void* stream) {
     switch (bn) {
       case 128: return launch_wgrad<128>(a, s);
       case 192: return launch_wgrad<128>(a, s);      // MN-major W is staged in 64-column atoms per warpgroup: 96 does not tile
-      case 256: return launch_wgrad<256>(a, s);
+      case 256: return launch_wgrad<128>(a, s);      // fp32 output tiles run at 128 columns (GemmCfg)
       default: return fail(PXA_ERR_ARG, "block_n must be 0, 128, 192 or 256 (got %d)", bn);
     }
   }
@@ -487,6 +631,7 @@ int gemm_bf16_rows(const PxaGemmArgs* args, int row_base, void* stream) {
   if ((ln_epi || a.aux_scale) && rpb < kBM && a.M > rpb)
     return fail(PXA_ERR_ARG, "the fused LayerNorm-modulate needs rows_per_batch >= %d (a tile may span two samples at most)", kBM);
   if (a.res_epilogue < 0 || a.res_epilogue > 2) return fail(PXA_ERR_ARG, "res_epilogue must be 0, 1 or 2");
+  if (bn == 256 && a.out_dtype == PXA_DTYPE_F32) bn = 128;   // fp32 output tiles run at 128 columns (GemmCfg)
   if (a.row_stats_out && (a.N + bn - 1) / bn > PXA_LN_STAT_PARTS)
     return fail(PXA_ERR_ARG, "row_stats_out: N / block_n = %d column tiles exceed PXA_LN_STAT_PARTS", (a.N + bn - 1) / bn);
   switch (bn) {

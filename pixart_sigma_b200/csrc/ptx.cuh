@@ -115,6 +115,18 @@ PXA_DEVICE void tma_reduce_add_2d(const CUtensorMap* map, const void* smem_src, 
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
                : "memory");
 }
+PXA_DEVICE void tma_store_3d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];\n" ::"l"(
+                   reinterpret_cast<uint64_t>(map)),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+PXA_DEVICE void tma_reduce_add_3d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];\n" ::"l"(
+                   reinterpret_cast<uint64_t>(map)),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
 // 1-D bulk copy shared -> global through the TMA engine (asynchronous, off the LSU): 16-byte aligned addresses, bytes % 16 == 0
 PXA_DEVICE void bulk_store_1d(void* gdst, const void* smem_src, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;\n" ::"l"(gdst), "r"(smem_u32(smem_src)), "r"(bytes) : "memory");
