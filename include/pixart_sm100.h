@@ -118,6 +118,24 @@ typedef struct PxaGemmArgs {
 } PxaGemmArgs;
 int pxa_gemm_bf16(const PxaGemmArgs* args, void* stream);
 
+/* ------------------------------------------------------------------------------------------- GEMM with a K-tail (LoRA)
+ * out = epilogue( A W^T + tail_a tail_w^T + bias ): the same kernel as pxa_gemm_bf16 with ceil(tail_k / 64) more K-blocks,
+ * read from tail_a [M, tail_k] and tail_w [N, tail_k] (bf16, K-contiguous) into the same operand ring after the last
+ * K-block of A W^T, so that the epilogue sees the sum.  Columns past tail_k are TMA zero fill.  For a LoRA projection
+ * tail_a = u = x A^T and tail_w = s B (block-diagonal over fused projections): the adapter's up-projection lands in the
+ * accumulator before the bias / GELU / gated-residual epilogue.  In the backward, tail_a = v = s dY B and tail_w = A^T.
+ * Accepts every PxaGemmArgs form except the fused LayerNorm epilogues (EPI_LN_*) and operands_mn_major
+ * (PXA_ERR_ARG); the convolution (pxa_conv3x3_nhwc_bf16) has no tail.  tail_k must be a multiple of 8 (PXA_ERR_ARG);
+ * tail_a / tail_w 16-byte aligned and lda_tail / ldw_tail multiples of 8 (PXA_ERR_ALIGN).  With a tail, block_n 256 runs at
+ * 192 and fp32 output at 128 (the wider tail instantiations would spill registers). */
+typedef struct PxaGemmTail {
+  const void* tail_a;   /* bf16 [M, tail_k], row stride lda_tail (elements) */
+  const void* tail_w;   /* bf16 [N, tail_k], row stride ldw_tail (elements) */
+  int32_t tail_k;
+  int32_t lda_tail, ldw_tail;
+} PxaGemmTail;
+int pxa_gemm_lora_bf16(const PxaGemmArgs* args, const PxaGemmTail* tail, void* stream);
+
 /* ------------------------------------------------------------------------------------------- fused Mlp
  * x32[r, :] += gate[b, :] * ( gelu_tanh(x[r, :] W1^T + b1) W2^T + b2 )        b = r / rows_per_batch
  * The timm Mlp of PixArtMSBlock with its gate and residual (PixArtMS.py:67,77), run in groups of `group` 256-row panels: per group

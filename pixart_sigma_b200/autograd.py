@@ -15,6 +15,12 @@ tape: every node below calls into libpixart_sm100.so in both directions --
                                                                                                 PixArt_blocks.py:52-53,153
   KvCompressFn    LN(conv2x2s2(k | v))    bwd: pxa_kv_compress_conv2_ln_bwd                       PixArt_blocks.py:97-121
 
+LoRA: a projection with an unmerged adapter (lora.py; operands from `lora.prepare_operands`) adds s u B^T with u = x A^T:
+u is a skinny GEMM (N = T), and the up-projection is a K-tail of the projection's own GEMM (`lib.gemm(tail_a=u,
+tail_w=s B)`), so every epilogue sees the sum.  Backward: v = s dY B (skinny GEMM), dX = dY W + v A (dgrad GEMM with the
+tail v, A^T), dA = v^T X and dB = s dY^T u (weight-gradient form, M = T), straight into lora_A.grad / lora_B.grad when they
+are bucket views.  Weights that do not require grad get no weight-gradient GEMM and no bias column sum.
+
 Parameters may be fp32 (mixed-precision training, `train.py:369` accelerator mixed_precision) or bf16; the kernels
 always consume bf16 shadows, cached per parameter version, and gradients are produced in fp32 and cast to the
 parameter dtype.  There is no eager fallback: a missing library or a non-sm_100 device raises from `lib`.
@@ -91,35 +97,109 @@ def clear_shadow_cache(model: torch.nn.Module) -> None:
         m.__dict__.pop("_pxa_shadow", None)
 
 
+def _lora_ops(mod):
+    """The adapter operands of `mod` for this training forward (lora.Operands), or None."""
+    return mod.__dict__.get("_pxa_lora")
+
+
+def _lora_params(mod):
+    """(lora_A, lora_B) of a projection with an active adapter, else (None, None): extra autograd inputs of its node."""
+    return (mod.lora_A, mod.lora_B) if _lora_ops(mod) is not None else (None, None)
+
+
+def _lora_u(x, mod):
+    """u = x A^T (bf16 [M, T]) for the forward tail, or None."""
+    op = _lora_ops(mod)
+    if op is None:
+        return None
+    return lib.gemm(x, op.a, None, torch.empty((x.shape[0], op.T), dtype=torch.bfloat16, device=x.device))
+
+
+def _lora_v(dy, mod, u):
+    """v = s dY B (bf16 [M, T]) for the dgrad tail, or None (no adapter: u is None)."""
+    if u is None:
+        return None
+    op = _lora_ops(mod)
+    return lib.gemm(dy, op.bt, None, torch.empty((dy.shape[0], op.T), dtype=torch.bfloat16, device=dy.device))
+
+
+def _tail(t, mod, kind: str) -> dict:
+    """gemm() arguments of the K-tail t [M, T] times the adapter operand `kind` of `mod` ("b" forward, "at" dgrad)."""
+    return {} if t is None else dict(tail_a=t, tail_w=getattr(_lora_ops(mod), kind))
+
+
+def _to_grad(p, g):
+    """Add the fp32 gradient g into p.grad when the kernels may accumulate there directly, else return it for autograd."""
+    acc = _grad_accumulator(p)
+    if acc is None:
+        return g if p.dtype == torch.float32 else g.to(p.dtype)
+    acc.add_(g)
+    _grad_landed(p)
+    return None
+
+
+def _lora_wgrad(mod, x, u, dy, v, needs):
+    """(dA, dB) of the adapter of `mod`: dA = v^T x and dB = s dY^T u on the diagonal blocks.  needs = (A, B)."""
+    op = _lora_ops(mod)
+    A, B = mod.lora_A, mod.lora_B
+    dA = dB = None
+    dev = x.device
+    GR = A.shape[0]
+    if needs[0]:
+        acc = _grad_accumulator(A)
+        if acc is not None and op.T == GR:
+            lib.gemm_wgrad(v, x, acc)                                          # straight into the bucket view
+            _grad_landed(A)
+        else:
+            g = torch.zeros((op.T, x.shape[1]), dtype=torch.float32, device=dev)
+            lib.gemm_wgrad(v, x, g)
+            dA = _to_grad(A, g[:GR])
+    if needs[1]:
+        G, Ng, r = B.shape
+        g = torch.zeros((op.T, dy.shape[1]), dtype=torch.float32, device=dev)  # u^T dY: only its diagonal blocks are used
+        lib.gemm_wgrad(u, dy, g)
+        blocks = g[:GR].view(G, r, G, Ng).diagonal(dim1=0, dim2=2).permute(2, 1, 0)    # [G, Ng, r]
+        dB = _to_grad(B, blocks * op.s)
+    return dA, dB
+
+
 class LinearFn(torch.autograd.Function):
-    """y = x W^T + b of `mod` (an nn.Linear: the owner of the bf16 shadows); weight / bias are passed as tensors too so
-    that autograd routes their gradients."""
+    """y = x W^T + b of `mod` (an nn.Linear: the owner of the bf16 shadows); weight / bias (and the adapter's lora_A /
+    lora_B) are passed as tensors too so that autograd routes their gradients."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, mod):
+    def forward(ctx, x, weight, bias, mod, lora_A=None, lora_B=None):
         assert x.dtype == torch.bfloat16 and x.dim() == 2
         x = x.contiguous()
         out = torch.empty((x.shape[0], weight.shape[0]), dtype=torch.bfloat16, device=x.device)
-        lib.gemm(x, _shadow(mod, "w"), _shadow(mod, "b"), out)
-        ctx.save_for_backward(x, weight, bias)
+        u = _lora_u(x, mod)
+        lib.gemm(x, _shadow(mod, "w"), _shadow(mod, "b"), out, **_tail(u, mod, "b"))
+        ctx.save_for_backward(x, weight, bias, u)
         ctx.mod = mod
         return out
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight, bias = ctx.saved_tensors
-        dx, dw, db = _linear_backward(ctx.needs_input_grad[:3], x, weight, bias, ctx.mod, dy.contiguous())
-        return dx, dw, db, None
+        x, weight, bias, u = ctx.saved_tensors
+        n = ctx.needs_input_grad
+        dx, dw, db, dA, dB = _linear_backward(n[:3], x, weight, bias, ctx.mod, dy.contiguous(), u=u, lora_needs=n[4:6])
+        return dx, dw, db, None, dA, dB
 
 
-def _linear_backward(ctx_needs, x, weight, bias, mod, dy):
-    """(dx, dw, db) of y = x W^T + b for the incoming dy (bf16, contiguous); ctx_needs = needs_input_grad of (x, W, b)."""
+def _linear_backward(ctx_needs, x, weight, bias, mod, dy, u=None, v=None, lora_needs=(False, False)):
+    """(dx, dw, db, dA, dB) of y = x W^T + b [+ s (x A^T) B^T] for the incoming dy (bf16, contiguous); ctx_needs =
+    needs_input_grad of (x, W, b), lora_needs of (A, B).  u = x A^T from the forward (None: no adapter); v = s dY B when
+    the caller already has it."""
     M, K = x.shape
     N = weight.shape[0]
-    dx = dw = db = None
+    dx = dw = db = dA = dB = None
+    lora = u is not None and (ctx_needs[0] or any(lora_needs))
+    if lora and v is None:
+        v = _lora_v(dy, mod, u)
     if ctx_needs[0]:
         dx = torch.empty((M, K), dtype=torch.bfloat16, device=x.device)
-        lib.gemm(dy, _shadow(mod, "t"), None, dx)                              # dX = dY . W   (W^T is K-contiguous in N)
+        # dX = dY . W (+ v A)   (W^T is K-contiguous in N)
+        lib.gemm(dy, _shadow(mod, "t"), None, dx, **_tail(v if lora else None, mod, "at"))
     if ctx_needs[1]:
         acc = _grad_accumulator(mod.weight)
         if acc is not None:
@@ -140,7 +220,9 @@ def _linear_backward(ctx_needs, x, weight, bias, mod, dy):
             db32 = torch.zeros((N,), dtype=torch.float32, device=x.device)
             lib.colsum(dy, db32)
             db = db32 if bias.dtype == torch.float32 else db32.to(bias.dtype)
-    return dx, dw, db
+    if lora and any(lora_needs):
+        dA, dB = _lora_wgrad(mod, x, u, dy, v, lora_needs)
+    return dx, dw, db, dA, dB
 
 
 def _grad_accumulator(p: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
@@ -168,22 +250,23 @@ class LinearGateResidualFn(torch.autograd.Function):
     gate's gradient is sum_rows dout * branch."""
 
     @staticmethod
-    def forward(ctx, a, weight, bias, mod, x32, tab, i_gate, rows_per_batch):
+    def forward(ctx, a, weight, bias, mod, x32, tab, i_gate, rows_per_batch, lora_A=None, lora_B=None):
         a, x32 = a.contiguous(), x32.contiguous()
         M, N = a.shape[0], weight.shape[0]
         out = torch.empty((M, N), dtype=torch.float32, device=a.device)
         gated = i_gate >= 0
         y = torch.empty((M, N), dtype=torch.bfloat16, device=a.device) if gated else None
+        u = _lora_u(a, mod)
         lib.gemm(a, _shadow(mod, "w"), _shadow(mod, "b"), out, epilogue=lib.EPI_BIAS_RESIDUAL, residual=x32,
                  gate=tab[:, i_gate] if gated else None, gate_batch_stride=tab.stride(0) if gated else 0,
-                 rows_per_batch=rows_per_batch, out_aux=y, aux_is_branch=True)
-        ctx.save_for_backward(a, weight, bias, y, tab if gated else None)
+                 rows_per_batch=rows_per_batch, out_aux=y, aux_is_branch=True, **_tail(u, mod, "b"))
+        ctx.save_for_backward(a, weight, bias, y, tab if gated else None, u)
         ctx.mod, ctx.idx = mod, (i_gate, rows_per_batch)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        a, weight, bias, y, tab = ctx.saved_tensors
+        a, weight, bias, y, tab, u = ctx.saved_tensors
         i_gate, rpb = ctx.idx
         dout = dout.contiguous()
         dy = torch.empty(dout.shape, dtype=torch.bfloat16, device=dout.device)
@@ -198,8 +281,9 @@ class LinearGateResidualFn(torch.autograd.Function):
                 dtab[:, i_gate] = dg
         else:
             lib.gate_residual_bwd(dout, None, None, dy, None, rows_per_batch=rpb)
-        da, dw, db = _linear_backward(ctx.needs_input_grad[:3], a, weight, bias, ctx.mod, dy)
-        return da, dw, db, None, dout, dtab, None, None
+        n = ctx.needs_input_grad
+        da, dw, db, dA, dB = _linear_backward(n[:3], a, weight, bias, ctx.mod, dy, u=u, lora_needs=n[8:10])
+        return da, dw, db, None, dout, dtab, None, None, dA, dB
 
 
 class MlpGateResidualFn(torch.autograd.Function):
@@ -209,23 +293,28 @@ class MlpGateResidualFn(torch.autograd.Function):
     gelu'(pre) in its epilogue (EPI_MUL_DGELU): no separate GELU forward / backward passes over the [M, 4C] hidden."""
 
     @staticmethod
-    def forward(ctx, xn, w1, b1, w2, b2, fc1, fc2, x32, tab, i_gate, rows_per_batch):
+    def forward(ctx, xn, w1, b1, w2, b2, fc1, fc2, x32, tab, i_gate, rows_per_batch, A1=None, B1=None, A2=None, B2=None):
         xn, x32 = xn.contiguous(), x32.contiguous()
         M, Hd, N = xn.shape[0], w1.shape[0], w2.shape[0]
         bf = dict(dtype=torch.bfloat16, device=xn.device)
         h, pre = torch.empty((M, Hd), **bf), torch.empty((M, Hd), **bf)
-        lib.gemm(xn, _shadow(fc1, "w"), _shadow(fc1, "b"), h, epilogue=lib.EPI_BIAS_GELU_AUX, out_aux=pre)
+        u1 = _lora_u(xn, fc1)
+        lib.gemm(xn, _shadow(fc1, "w"), _shadow(fc1, "b"), h, epilogue=lib.EPI_BIAS_GELU_AUX, out_aux=pre,
+                 **_tail(u1, fc1, "b"))
         out = torch.empty((M, N), dtype=torch.float32, device=xn.device)
         y = torch.empty((M, N), **bf)
+        u2 = _lora_u(h, fc2)
         lib.gemm(h, _shadow(fc2, "w"), _shadow(fc2, "b"), out, epilogue=lib.EPI_BIAS_RESIDUAL, residual=x32, gate=tab[:, i_gate],
-                 gate_batch_stride=tab.stride(0), rows_per_batch=rows_per_batch, out_aux=y, aux_is_branch=True)
-        ctx.save_for_backward(xn, pre, h, y, tab, w1, b1, w2, b2)
+                 gate_batch_stride=tab.stride(0), rows_per_batch=rows_per_batch, out_aux=y, aux_is_branch=True,
+                 **_tail(u2, fc2, "b"))
+        ctx.save_for_backward(xn, pre, h, y, tab, w1, b1, w2, b2, u1, u2)
         ctx.mods, ctx.idx = (fc1, fc2), (i_gate, rows_per_batch)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        xn, pre, h, y, tab, w1, b1, w2, b2 = ctx.saved_tensors
+        xn, pre, h, y, tab, w1, b1, w2, b2, u1, u2 = ctx.saved_tensors
+        n = ctx.needs_input_grad
         fc1, fc2 = ctx.mods
         i_gate, rpb = ctx.idx
         dout = dout.contiguous()
@@ -238,11 +327,13 @@ class MlpGateResidualFn(torch.autograd.Function):
         if want:
             dtab = torch.zeros_like(tab)
             dtab[:, i_gate] = dg
-        _, dw2, db2 = _linear_backward((False, True, True), h, w2, b2, fc2, dy)
+        v2 = _lora_v(dy, fc2, u2)
+        _, dw2, db2, dA2, dB2 = _linear_backward((False, n[3], n[4]), h, w2, b2, fc2, dy, u=u2, v=v2, lora_needs=n[13:15])
         dpre = torch.empty_like(pre)
-        lib.gemm(dy, _shadow(fc2, "t"), None, dpre, epilogue=lib.EPI_MUL_DGELU, residual=pre)     # dh * gelu'(pre) in the epilogue
-        dxn, dw1, db1 = _linear_backward((True, True, True), xn, w1, b1, fc1, dpre)
-        return dxn, dw1, db1, dw2, db2, None, None, dout, dtab, None, None
+        lib.gemm(dy, _shadow(fc2, "t"), None, dpre, epilogue=lib.EPI_MUL_DGELU, residual=pre,     # dh * gelu'(pre) in the epilogue
+                 **_tail(v2, fc2, "at"))
+        dxn, dw1, db1, dA1, dB1 = _linear_backward((True, n[1], n[2]), xn, w1, b1, fc1, dpre, u=u1, lora_needs=n[11:13])
+        return dxn, dw1, db1, dw2, db2, None, None, dout, dtab, None, None, dA1, dB1, dA2, dB2
 
 
 class LnModulateFn(torch.autograd.Function):
@@ -488,7 +579,7 @@ class CrossAttnFn(torch.autograd.Function):
 
 
 def linear(x: torch.Tensor, mod: torch.nn.Linear) -> torch.Tensor:
-    return LinearFn.apply(x, mod.weight, mod.bias, mod)
+    return LinearFn.apply(x, mod.weight, mod.bias, mod, *_lora_params(mod))
 
 
 def _compressed_self_attention(a, qkv: torch.Tensor, B: int, H: int, N: int, HW) -> torch.Tensor:
@@ -529,19 +620,20 @@ def block_forward_train(blk, x32: torch.Tensor, cond: torch.Tensor, kv_len: Opti
         ao = _compressed_self_attention(a, _qk_norm(a, linear(xn, a.qkv)), B, H, N, HW)
     else:
         ao = SelfAttnFn.apply(_qk_norm(a, linear(xn, a.qkv)), B, H, N, a.scale, keep, _fp32_p(a))
-    x32 = LinearGateResidualFn.apply(ao, a.proj.weight, a.proj.bias, a.proj, x32, mod, 2, N)
+    x32 = LinearGateResidualFn.apply(ao, a.proj.weight, a.proj.bias, a.proj, x32, mod, 2, N, *_lora_params(a.proj))
     # (2) x += proj(cross_attn(x, cond))                                                          PixArtMS.py:76
     qx = linear(x32.to(torch.bfloat16), ca.q_linear)
     kv = linear(cond, ca.kv_linear)
     ao = CrossAttnFn.apply(qx, kv, kv_len, kv_off, B, H, N, max_keys, ca.head_dim ** -0.5, keep)
-    x32 = LinearGateResidualFn.apply(ao, ca.proj.weight, ca.proj.bias, ca.proj, x32, mod, -1, N)
+    x32 = LinearGateResidualFn.apply(ao, ca.proj.weight, ca.proj.bias, ca.proj, x32, mod, -1, N, *_lora_params(ca.proj))
     # (3) x += gate_mlp * fc2(gelu_tanh(fc1(LN(x) * (1 + scale_mlp) + shift_mlp)))               PixArtMS.py:77
     xn = LnModulateFn.apply(x32, mod, 3, 4, N)
     if _FUSED_MLP:                                    # experimental, see MlpGateResidualFn
-        x32 = MlpGateResidualFn.apply(xn, mlp.fc1.weight, mlp.fc1.bias, mlp.fc2.weight, mlp.fc2.bias, mlp.fc1, mlp.fc2, x32, mod, 5, N)
+        x32 = MlpGateResidualFn.apply(xn, mlp.fc1.weight, mlp.fc1.bias, mlp.fc2.weight, mlp.fc2.bias, mlp.fc1, mlp.fc2, x32, mod, 5, N,
+                                      *_lora_params(mlp.fc1), *_lora_params(mlp.fc2))
     else:
         h = GeluFn.apply(linear(xn, mlp.fc1))
-        x32 = LinearGateResidualFn.apply(h, mlp.fc2.weight, mlp.fc2.bias, mlp.fc2, x32, mod, 5, N)
+        x32 = LinearGateResidualFn.apply(h, mlp.fc2.weight, mlp.fc2.bias, mlp.fc2, x32, mod, 5, N, *_lora_params(mlp.fc2))
     if keep is not None:
         keep["replay"] = True            # the next call with this dict is the recomputation
     return x32
@@ -551,24 +643,36 @@ def block_forward_train(blk, x32: torch.Tensor, cond: torch.Tensor, kv_len: Opti
 _BLOCK_FN = os.environ.get("PXA_BLOCK_FN", "1") == "1"
 
 
+_TAGS = ("qkv", "proj", "q", "kv", "cproj", "fc1", "fc2")
+
+
 def _block_params(blk):
+    """The block's projections in _TAGS order and, per projection, (weight, bias, lora_A, lora_B) (None: no adapter)."""
     a, ca, mlp = blk.attn, blk.cross_attn, blk.mlp
     mods = (a.qkv, a.proj, ca.q_linear, ca.kv_linear, ca.proj, mlp.fc1, mlp.fc2)
-    return mods, tuple(t for m in mods for t in (m.weight, m.bias))
+    return mods, tuple(t for m in mods for t in (m.weight, m.bias, *_lora_params(m)))
 
 
 def _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, kept=None):
     """The block's forward on the kernels, out of place, returning every intermediate the backward reads.  `kept` = the two
-    attention outputs + softmax statistics of an earlier pass (activation checkpointing: they are not recomputed)."""
+    attention outputs + softmax statistics of an earlier pass and its adapter down-projections u_<tag> (activation
+    checkpointing: they are not recomputed)."""
     a, ca, mlp = blk.attn, blk.cross_attn, blk.mlp
     C, H = blk.hidden_size, a.num_heads
     D, M, dev = C // H, B * N, x32.device
     bf = dict(dtype=torch.bfloat16, device=dev)
     f32 = dict(dtype=torch.float32, device=dev)
     ms = mod.stride(0)
-    t = {}
+    t = {k: v for k, v in kept.items() if k.startswith("u_")} if kept is not None else {}
+
+    def gemm(tag, x, lin, out, **kw):
+        """The projection `lin` (tag in _TAGS) with its adapter's up-projection as the K-tail; u_<tag> kept in t."""
+        if _lora_ops(lin) is not None and "u_" + tag not in t:
+            t["u_" + tag] = _lora_u(x, lin)
+        return lib.gemm(x, _shadow(lin, "w"), _shadow(lin, "b"), out, **kw, **_tail(t.get("u_" + tag), lin, "b"))
+
     t["xn1"] = lib.ln_modulate(x32, mod[:, 0], mod[:, 1], torch.empty((M, C), **bf), mod_batch_stride=ms, rows_per_batch=N)
-    t["qkv"] = lib.gemm(t["xn1"], _shadow(a.qkv, "w"), _shadow(a.qkv, "b"), torch.empty((M, 3 * C), **bf))
+    t["qkv"] = gemm("qkv", t["xn1"], a.qkv, torch.empty((M, 3 * C), **bf))
     q3 = t["qkv"].view(M, 3, H, D)
     st = (3 * C, D)
     if kept is None:
@@ -576,13 +680,13 @@ def _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, 
         lib.flash_attn(q3[:, 0], q3[:, 1], q3[:, 2], t["ao1"], B=B, H=H, Nq=N, Nk=N, kv_rows=M, q_strides=st, k_strides=st,
                        v_strides=st, scale=a.scale, lse=t["lse1"], fp32_p=_fp32_p(a))
     else:
-        t["ao1"], t["lse1"] = kept[0], kept[1]
+        t["ao1"], t["lse1"] = kept["ao1"], kept["lse1"]
     t["x1"], t["y1"] = torch.empty((M, C), **f32), torch.empty((M, C), **bf)
-    lib.gemm(t["ao1"], _shadow(a.proj, "w"), _shadow(a.proj, "b"), t["x1"], epilogue=lib.EPI_BIAS_RESIDUAL, residual=x32,
-             gate=mod[:, 2], gate_batch_stride=ms, rows_per_batch=N, out_aux=t["y1"], aux_is_branch=True)
+    gemm("proj", t["ao1"], a.proj, t["x1"], epilogue=lib.EPI_BIAS_RESIDUAL, residual=x32, gate=mod[:, 2], gate_batch_stride=ms,
+         rows_per_batch=N, out_aux=t["y1"], aux_is_branch=True)
     t["xb"] = t["x1"].to(torch.bfloat16)
-    t["qx"] = lib.gemm(t["xb"], _shadow(ca.q_linear, "w"), _shadow(ca.q_linear, "b"), torch.empty((M, C), **bf))
-    t["kv"] = lib.gemm(cond, _shadow(ca.kv_linear, "w"), _shadow(ca.kv_linear, "b"), torch.empty((cond.shape[0], 2 * C), **bf))
+    t["qx"] = gemm("q", t["xb"], ca.q_linear, torch.empty((M, C), **bf))
+    t["kv"] = gemm("kv", cond, ca.kv_linear, torch.empty((cond.shape[0], 2 * C), **bf))
     kv4 = t["kv"].view(-1, 2, H, D)
     if kept is None:
         t["ao2"], t["lse2"] = torch.empty((M, C), **bf), torch.empty((B, H, N), **f32)
@@ -590,17 +694,16 @@ def _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, 
                        kv_off=kv_off, q_strides=(C, D), k_strides=(2 * C, D), v_strides=(2 * C, D), scale=ca.head_dim ** -0.5,
                        lse=t["lse2"])
     else:
-        t["ao2"], t["lse2"] = kept[2], kept[3]
+        t["ao2"], t["lse2"] = kept["ao2"], kept["lse2"]
     t["x2"] = torch.empty((M, C), **f32)
-    lib.gemm(t["ao2"], _shadow(ca.proj, "w"), _shadow(ca.proj, "b"), t["x2"], epilogue=lib.EPI_BIAS_RESIDUAL, residual=t["x1"],
-             rows_per_batch=N)
+    gemm("cproj", t["ao2"], ca.proj, t["x2"], epilogue=lib.EPI_BIAS_RESIDUAL, residual=t["x1"], rows_per_batch=N)
     t["xn2"] = lib.ln_modulate(t["x2"], mod[:, 3], mod[:, 4], torch.empty((M, C), **bf), mod_batch_stride=ms, rows_per_batch=N)
     Hd = mlp.fc1.out_features
     t["h"], t["pre"] = torch.empty((M, Hd), **bf), torch.empty((M, Hd), **bf)
-    lib.gemm(t["xn2"], _shadow(mlp.fc1, "w"), _shadow(mlp.fc1, "b"), t["h"], epilogue=lib.EPI_BIAS_GELU_AUX, out_aux=t["pre"])
+    gemm("fc1", t["xn2"], mlp.fc1, t["h"], epilogue=lib.EPI_BIAS_GELU_AUX, out_aux=t["pre"])
     t["x3"], t["y3"] = torch.empty((M, C), **f32), torch.empty((M, C), **bf)
-    lib.gemm(t["h"], _shadow(mlp.fc2, "w"), _shadow(mlp.fc2, "b"), t["x3"], epilogue=lib.EPI_BIAS_RESIDUAL, residual=t["x2"],
-             gate=mod[:, 5], gate_batch_stride=ms, rows_per_batch=N, out_aux=t["y3"], aux_is_branch=True)
+    gemm("fc2", t["h"], mlp.fc2, t["x3"], epilogue=lib.EPI_BIAS_RESIDUAL, residual=t["x2"], gate=mod[:, 5], gate_batch_stride=ms,
+         rows_per_batch=N, out_aux=t["y3"], aux_is_branch=True)
     return t
 
 
@@ -624,22 +727,20 @@ class BlockFn(torch.autograd.Function):
     def forward(ctx, blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, ckpt, *params):
         x32, cond, mod = x32.contiguous(), cond.contiguous(), mod.contiguous()
         t = _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N)
-        names = _KEPT if ckpt else _SAVED
+        names = (_KEPT if ckpt else _SAVED) + tuple(k for k in t if k.startswith("u_"))
         ctx.save_for_backward(x32, cond, mod, kv_len, kv_off, *[t[k] for k in names], *params)
-        ctx.meta = (blk, max_keys, B, N, bool(ckpt), len(names))
+        ctx.meta = (blk, max_keys, B, N, bool(ckpt), names)
         return t["x3"]
 
     @staticmethod
     def backward(ctx, dout):
-        blk, max_keys, B, N, ckpt, n_names = ctx.meta
+        blk, max_keys, B, N, ckpt, names = ctx.meta
         saved = ctx.saved_tensors
         x32, cond, mod, kv_len, kv_off = saved[:5]
-        vals = saved[5:5 + n_names]
-        params = saved[5 + n_names:]
+        t = dict(zip(names, saved[5:5 + len(names)]))
+        params = saved[5 + len(names):]
         if ckpt:
-            t = _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, kept=vals)
-        else:
-            t = dict(zip(_SAVED, vals))
+            t = _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, kept=t)
         a, ca, mlp = blk.attn, blk.cross_attn, blk.mlp
         C, H = blk.hidden_size, a.num_heads
         D, M, dev = C // H, B * N, x32.device
@@ -648,51 +749,56 @@ class BlockFn(torch.autograd.Function):
         ms = mod.stride(0)
         dout = dout.contiguous()
         dm = torch.zeros((6, B, C), **f32)                # d(shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp)
-        (w_qkv, b_qkv, w_p, b_p, w_q, b_q, w_kv, b_kv, w_cp, b_cp, w_1, b_1, w_2, b_2) = params
+        needs = ctx.needs_input_grad[10:]
         grads = {}
 
-        def lin_bwd(tag, x, weight, bias, lin_mod, dy, need_dx=True):
-            dx, dw, db = _linear_backward((need_dx, True, True), x, weight, bias, lin_mod, dy)
-            grads[tag] = (dw, db)
+        def lin_bwd(tag, x, lin_mod, dy, need_dx=True, v=None):
+            i = _TAGS.index(tag)
+            weight, bias = params[4 * i], params[4 * i + 1]
+            n = needs[4 * i:4 * i + 4]
+            dx, *g = _linear_backward((need_dx, n[0], n[1]), x, weight, bias, lin_mod, dy, u=t.get("u_" + tag), v=v,
+                                      lora_needs=n[2:])
+            grads[tag] = g
             return dx
 
         # (3) x3 = x2 + gate_mlp * (fc2(gelu(fc1(xn2))) + b2)
         dy3 = torch.empty((M, C), **bf)
         lib.gate_residual_bwd(dout, t["y3"], mod[:, 5], dy3, dm[5], gate_batch_stride=ms, rows_per_batch=N)
-        lin_bwd("fc2", t["h"], w_2, b_2, mlp.fc2, dy3, need_dx=False)
+        v2 = _lora_v(dy3, mlp.fc2, t.get("u_fc2"))
+        lin_bwd("fc2", t["h"], mlp.fc2, dy3, need_dx=False, v=v2)
         dpre = torch.empty_like(t["pre"])
-        lib.gemm(dy3, _shadow(mlp.fc2, "t"), None, dpre, epilogue=lib.EPI_MUL_DGELU, residual=t["pre"])
-        dxn2 = lin_bwd("fc1", t["xn2"], w_1, b_1, mlp.fc1, dpre)
+        lib.gemm(dy3, _shadow(mlp.fc2, "t"), None, dpre, epilogue=lib.EPI_MUL_DGELU, residual=t["pre"], **_tail(v2, mlp.fc2, "at"))
+        dxn2 = lin_bwd("fc1", t["xn2"], mlp.fc1, dpre)
         dx2 = torch.empty((M, C), **f32)                  # = dout (the residual path) + the gradient through norm2
         lib.ln_modulate_bwd(t["x2"], dxn2, mod[:, 4], dx2, dm[3], dm[4], mod_batch_stride=ms, rows_per_batch=N, add_in=dout)
         # (2) x2 = x1 + cross_proj(cross_attn(q_linear(bf16(x1)), kv_linear(cond)))
         dy2 = torch.empty((M, C), **bf)
         lib.gate_residual_bwd(dx2, None, None, dy2, None, rows_per_batch=N)
-        dao2 = lin_bwd("cproj", t["ao2"], w_cp, b_cp, ca.proj, dy2)
+        dao2 = lin_bwd("cproj", t["ao2"], ca.proj, dy2)
         dq, dkv = torch.empty((M, C), **bf), torch.zeros_like(t["kv"])      # padding key rows get no gradient
         kv4, d4 = t["kv"].view(-1, 2, H, D), dkv.view(-1, 2, H, D)
         lib.flash_attn_bwd(t["qx"], kv4[:, 0], kv4[:, 1], t["ao2"], dao2, t["lse2"], dq, d4[:, 0], d4[:, 1], B=B, H=H, Nq=N,
                            Nk=max_keys, kv_rows=t["kv"].shape[0], kv_len=kv_len, kv_off=kv_off, q_strides=(C, D),
                            k_strides=(2 * C, D), v_strides=(2 * C, D), dq_strides=(C, D), dk_strides=(2 * C, D),
                            dv_strides=(2 * C, D), scale=ca.head_dim ** -0.5)
-        dxb = lin_bwd("q", t["xb"], w_q, b_q, ca.q_linear, dq)
-        dcond = lin_bwd("kv", cond, w_kv, b_kv, ca.kv_linear, dkv)
+        dxb = lin_bwd("q", t["xb"], ca.q_linear, dq)
+        dcond = lin_bwd("kv", cond, ca.kv_linear, dkv)
         dx1 = torch.empty((M, C), **f32)
         lib.gate_residual_fwd(dx2, dxb, None, dx1, rows_per_batch=N)          # dx1 = dx2 + float(dxb)
         # (1) x1 = x + gate_msa * (proj(attn(qkv(xn1))) + b)
         dy1 = torch.empty((M, C), **bf)
         lib.gate_residual_bwd(dx1, t["y1"], mod[:, 2], dy1, dm[2], gate_batch_stride=ms, rows_per_batch=N)
-        dao1 = lin_bwd("proj", t["ao1"], w_p, b_p, a.proj, dy1)
+        dao1 = lin_bwd("proj", t["ao1"], a.proj, dy1)
         dqkv = torch.empty_like(t["qkv"])
         q3, g3 = t["qkv"].view(M, 3, H, D), dqkv.view(M, 3, H, D)
         st = (3 * C, D)
         lib.flash_attn_bwd(q3[:, 0], q3[:, 1], q3[:, 2], t["ao1"], dao1, t["lse1"], g3[:, 0], g3[:, 1], g3[:, 2], B=B, H=H, Nq=N,
                            Nk=N, kv_rows=M, q_strides=st, k_strides=st, v_strides=st, dq_strides=st, dk_strides=st, dv_strides=st,
                            scale=a.scale)
-        dxn1 = lin_bwd("qkv", t["xn1"], w_qkv, b_qkv, a.qkv, dqkv)
+        dxn1 = lin_bwd("qkv", t["xn1"], a.qkv, dqkv)
         dx = torch.empty((M, C), **f32)
         lib.ln_modulate_bwd(x32, dxn1, mod[:, 1], dx, dm[0], dm[1], mod_batch_stride=ms, rows_per_batch=N, add_in=dx1)
-        pg = [g for tag in ("qkv", "proj", "q", "kv", "cproj", "fc1", "fc2") for g in grads[tag]]
+        pg = [g for tag in _TAGS for g in grads[tag]]
         return (None, dx, dcond, dm.permute(1, 0, 2), None, None, None, None, None, None, *pg)
 
 

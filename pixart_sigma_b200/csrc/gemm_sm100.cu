@@ -16,10 +16,21 @@
 // Tiles are visited n-fastest so the CTAs running concurrently share the same few A row-blocks through L2 and the
 // whole weight matrix stays L2-resident.
 //
+// K-tail (kTail, pxa_gemm_lora_bf16): after the tile's last K-block of A W^T the producer loads ceil(tail_k / 64) more
+// K-blocks from the tail operands (tail_a [M, tail_k], tail_w [N, tail_k]) into the same ring, and the consumers run the same
+// wgmma loop over them: the epilogue sees A W^T + tail_a tail_w^T.  TMA zero-fills the columns past tail_k.
+//
 // Algorithmic work: 2*M*N*K FLOP; bytes: M*K*2 (A) + N*K*2 (W) + M*N*out bytes (+ residual read).
 #include "gemm_common.cuh"
 
 namespace pxa {
+
+// Tensor maps of the K-tail operands; empty in the instantiations without a tail.
+template <bool kTail> struct TailMaps {
+  CUtensorMap a, w;
+  int num_kb;
+};
+template <> struct TailMaps<false> {};
 
 // K-block of a tile (counted from the tile's first) after which the consumers release the output tile of the previous tile:
 // late enough for its stores to have drained, early enough for the next operand to arrive before the tile's epilogue.
@@ -39,10 +50,11 @@ PXA_DEVICE int release_kb(int nk) {
 // tmap_out / tmap_res: `out` and the epilogue operand as 3-D tensors (column, x, line) with 32 x 128 x 1 boxes.  x runs over
 // the GEMM rows (one line), except for a convolution over a virtual width, where it runs over the W real pixels of an image
 // line: the stores drop the columns x >= W and the rows >= M.
-template <int BN, int EPI, typename OutT, bool kConv = false, bool kMn = false>
+template <int BN, int EPI, typename OutT, bool kConv = false, bool kMn = false, bool kTail = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
-                 const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_res, const GemmParams p) {
+                 const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_res, const GemmParams p,
+                 const __grid_constant__ TailMaps<kTail> tail) {
   constexpr bool kF32Res = (EPI == PXA_EPI_BIAS_RESIDUAL) && sizeof(OutT) == 4;
   constexpr bool kRes = EPI == PXA_EPI_BIAS_RESIDUAL;
   constexpr bool kLn = (EPI == PXA_EPI_LN_BIAS || EPI == PXA_EPI_LN_BIAS_GELU);
@@ -51,6 +63,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   constexpr int NW = BN / 2;                       // columns per consumer warpgroup
   constexpr int kSlabs = NW / 32;                  // output slabs per consumer warpgroup
   static_assert(!kMn || NW % 64 == 0, "MN-major W is staged in 64-column atoms");
+  static_assert(!kTail || (!kConv && !kMn && !kLn), "the K-tail belongs to the K-major, non-LayerNorm forms");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* otile = smem + kStages * Cfg::kStage;                                  // output tile: slab cs at cs * kSlabBytes
@@ -69,6 +82,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_w);
     prefetch_tmap(&tmap_out);
+    if constexpr (kTail) {
+      prefetch_tmap(&tail.a);
+      prefetch_tmap(&tail.w);
+    }
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], kNumEpiThreads / 32);
@@ -82,6 +99,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int mn_tiles = p.num_m_tiles * p.num_n_tiles;
   const int num_tiles = mn_tiles * p.k_splits;
   const int num_kb = (p.K + kBK - 1) / kBK;
+  int tail_kb = 0;                              // K-blocks of the tail, after the last K-block of every tile (k_splits == 1)
+  if constexpr (kTail) tail_kb = tail.num_kb;
   // tile -> (k split, m tile, n tile), n fastest; K-blocks [kb_lo, kb_hi) of split ks
   auto eff = [&](int tile) { return p.reverse_tiles ? num_tiles - 1 - tile : tile; };
   auto kb_lo = [&](int tile) { return (int)((long long)(tile / mn_tiles) * num_kb / p.k_splits); };
@@ -110,7 +129,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         const int tile = eff(t);
         const int m0 = tile_m0(tile);
         const int n0 = tile_n0(tile);
-        const int kb0 = kb_lo(tile), kb1 = kb_hi(tile);
+        const int kb0 = kb_lo(tile), kb1 = kb_hi(tile) + tail_kb;
         const int rel = release_kb(kb1 - kb0);
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -123,6 +142,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 #pragma unroll
             for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, &tmap_w, &full_bar[stage], n0 + 64 * j, kb * kBK, kEvictNormal);
           } else {
+            const CUtensorMap* ma = &tmap_a;
+            const CUtensorMap* mw = &tmap_w;
+            int kc = kb;                                              // K-block within its operand pair
+            if constexpr (kTail) {
+              if (kb >= num_kb) { ma = &tail.a; mw = &tail.w; kc = kb - num_kb; }
+            }
             if constexpr (kConv) {
               // implicit GEMM: K-block kb = (tap, 64-channel slice); the A tile is the tile's pixel block shifted by the
               // tap offset -- zero padding comes for free from TMA out-of-bounds fill on the W / H dimensions
@@ -134,9 +159,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
               const int b0 = pix / (p.conv_Wp * p.conv_H);
               tma_load_4d(sa, &tmap_a, &full_bar[stage], c0, x0 + tap % 3 - 1, y0 + tap / 3 - 1, b0, kEvictNormal);
             } else {
-              tma_load_2d(sa, &tmap_a, &full_bar[stage], kb * kBK, m0, kEvictNormal);
+              tma_load_2d(sa, ma, &full_bar[stage], kc * kBK, m0, kEvictNormal);
             }
-            tma_load_2d(sb, &tmap_w, &full_bar[stage], kb * kBK, n0, kEvictLast);
+            tma_load_2d(sb, mw, &full_bar[stage], kc * kBK, n0, kEvictLast);
           }
           if (++stage == kStages) { stage = 0; phase ^= 1; }
           if (has_opnd && kb - kb0 == rel) {
@@ -176,7 +201,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       // ---- main loop
       // One wgmma group stays in flight: the group of K-block kb is committed before the group of kb - 1 is waited for, and a
       // stage goes back to the producer once the group that read it has completed.
-      const int kb0 = kb_lo(tile), kb1 = kb_hi(tile);
+      const int kb0 = kb_lo(tile), kb1 = kb_hi(tile) + tail_kb;
       const int rel = release_kb(kb1 - kb0);
       int prev_stage = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
@@ -388,8 +413,9 @@ struct ConvGeom {
   int Wp;          // virtual width of the M index (= W when W tiles; else W rounded up to 128, see GemmParams::conv_Wp)
 };
 
-template <int BN, int EPI, typename OutT, bool kConv = false, bool kMn = false>
-static int launch_gemm(const GemmCall& a, cudaStream_t stream, const ConvGeom* cg = nullptr, int k_splits = 1) {
+template <int BN, int EPI, typename OutT, bool kConv = false, bool kMn = false, bool kTail = false>
+static int launch_gemm(const GemmCall& a, cudaStream_t stream, const ConvGeom* cg = nullptr, int k_splits = 1,
+                       const PxaGemmTail* tl = nullptr) {
   CUtensorMap ta, tw;
   if constexpr (kMn) {
     // A stored [K, M] (row stride lda), W stored [K, N] (row stride ldw): 64 x 64 boxes, M / N the contiguous dimension
@@ -441,6 +467,17 @@ static int launch_gemm(const GemmCall& a, cudaStream_t stream, const ConvGeom* c
       if (rc) return rc;
     }
   }
+  TailMaps<kTail> tm;
+  if constexpr (kTail) {
+    uint64_t dims_a[2] = {(uint64_t)tl->tail_k, (uint64_t)a.M}, dims_w[2] = {(uint64_t)tl->tail_k, (uint64_t)a.N};
+    uint64_t str_a[1] = {(uint64_t)tl->lda_tail * 2}, str_w[1] = {(uint64_t)tl->ldw_tail * 2};
+    uint32_t box_a[2] = {kBK, kBM}, box_w[2] = {kBK, (uint32_t)BN};
+    int rc = make_tmap_bf16(&tm.a, tl->tail_a, 2, dims_a, str_a, box_a, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    rc = make_tmap_bf16(&tm.w, tl->tail_w, 2, dims_w, str_w, box_w, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    tm.num_kb = (tl->tail_k + kBK - 1) / kBK;
+  }
   using Cfg = GemmCfg<BN, OutT>;
   GemmParams p = {};
   p.bias = reinterpret_cast<const __nv_bfloat16*>(a.bias);
@@ -463,39 +500,44 @@ static int launch_gemm(const GemmCall& a, cudaStream_t stream, const ConvGeom* c
     p.conv_cin_blocks = cg->Cin / kBK;
   }
   p.conv_Wp = kConv ? cg->Wp : 0;
-  auto kern = gemm_bf16_kernel<BN, EPI, OutT, kConv, kMn>;
+  auto kern = gemm_bf16_kernel<BN, EPI, OutT, kConv, kMn, kTail>;
   PXA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   int grid = device_info().sms;
   if (a.max_ctas > 0 && a.max_ctas < grid) grid = a.max_ctas;
   const int tiles = p.num_m_tiles * p.num_n_tiles * p.k_splits;
   if (tiles < grid) grid = tiles;
-  kern<<<grid, kGemmThreads, Cfg::kSmem, stream>>>(ta, tw, to, tr, p);
+  kern<<<grid, kGemmThreads, Cfg::kSmem, stream>>>(ta, tw, to, tr, p, tm);
   launch_counter()++;
   PXA_CHECK_CUDA(cudaGetLastError());
   return PXA_OK;
 }
 
-template <int BN>
-static int dispatch_epi(const GemmCall& a, cudaStream_t s) {
+template <int BN, bool kTail = false>
+static int dispatch_epi(const GemmCall& a, cudaStream_t s, const PxaGemmTail* tl = nullptr) {
   switch (a.epilogue) {
     case PXA_EPI_BIAS:
       if (a.out_dtype != PXA_DTYPE_BF16) return fail(PXA_ERR_ARG, "EPI_BIAS writes bf16 only");
-      return launch_gemm<BN, PXA_EPI_BIAS, __nv_bfloat16>(a, s);
+      return launch_gemm<BN, PXA_EPI_BIAS, __nv_bfloat16, false, false, kTail>(a, s, nullptr, 1, tl);
     case PXA_EPI_BIAS_GELU:
       if (a.out_dtype != PXA_DTYPE_BF16) return fail(PXA_ERR_ARG, "EPI_BIAS_GELU writes bf16 only");
-      return launch_gemm<BN, PXA_EPI_BIAS_GELU, __nv_bfloat16>(a, s);
+      return launch_gemm<BN, PXA_EPI_BIAS_GELU, __nv_bfloat16, false, false, kTail>(a, s, nullptr, 1, tl);
     case PXA_EPI_BIAS_GELU_AUX:
-      return launch_gemm<BN, PXA_EPI_BIAS_GELU_AUX, __nv_bfloat16>(a, s);
+      return launch_gemm<BN, PXA_EPI_BIAS_GELU_AUX, __nv_bfloat16, false, false, kTail>(a, s, nullptr, 1, tl);
     case PXA_EPI_MUL_DGELU:
-      return launch_gemm<BN, PXA_EPI_MUL_DGELU, __nv_bfloat16>(a, s);
+      return launch_gemm<BN, PXA_EPI_MUL_DGELU, __nv_bfloat16, false, false, kTail>(a, s, nullptr, 1, tl);
     case PXA_EPI_LN_BIAS:
-      return launch_gemm<BN, PXA_EPI_LN_BIAS, __nv_bfloat16>(a, s);
     case PXA_EPI_LN_BIAS_GELU:
-      return launch_gemm<BN, PXA_EPI_LN_BIAS_GELU, __nv_bfloat16>(a, s);
+      if constexpr (kTail) {
+        return fail(PXA_ERR_ARG, "the K-tail does not take the fused LayerNorm epilogues");
+      } else {
+        if (a.epilogue == PXA_EPI_LN_BIAS) return launch_gemm<BN, PXA_EPI_LN_BIAS, __nv_bfloat16>(a, s);
+        return launch_gemm<BN, PXA_EPI_LN_BIAS_GELU, __nv_bfloat16>(a, s);
+      }
     case PXA_EPI_BIAS_RESIDUAL:
       if (a.residual == nullptr) return fail(PXA_ERR_ARG, "EPI_BIAS_RESIDUAL needs residual");
-      if (a.out_dtype == PXA_DTYPE_F32) return launch_gemm<BN == 256 ? 128 : BN, PXA_EPI_BIAS_RESIDUAL, float>(a, s);
-      return launch_gemm<BN, PXA_EPI_BIAS_RESIDUAL, __nv_bfloat16>(a, s);
+      if (a.out_dtype == PXA_DTYPE_F32)
+        return launch_gemm<(BN == 256 || kTail) ? 128 : BN, PXA_EPI_BIAS_RESIDUAL, float, false, false, kTail>(a, s, nullptr, 1, tl);
+      return launch_gemm<BN, PXA_EPI_BIAS_RESIDUAL, __nv_bfloat16, false, false, kTail>(a, s, nullptr, 1, tl);
     default:
       return fail(PXA_ERR_ARG, "unknown epilogue %d", a.epilogue);
   }
@@ -572,7 +614,7 @@ extern "C" int pxa_conv3x3_nhwc_bf16(const PxaConv3x3Args* args, void* stream) {
 }
 
 namespace pxa {
-int gemm_bf16_rows(const PxaGemmArgs* args, int row_base, void* stream) {
+static int gemm_impl(const PxaGemmArgs* args, int row_base, const PxaGemmTail* tl, void* stream) {
   if (!args) return fail(PXA_ERR_ARG, "null args");
   GemmCall a;
   static_cast<PxaGemmArgs&>(a) = *args;
@@ -589,6 +631,18 @@ int gemm_bf16_rows(const PxaGemmArgs* args, int row_base, void* stream) {
        reinterpret_cast<uintptr_t>(a.out_aux_bf16)) & 15)
     return fail(PXA_ERR_ALIGN, "out / bias / residual / gate / aux must be 16-byte aligned");
   if (a.gate && (a.gate_batch_stride & 3)) return fail(PXA_ERR_ALIGN, "gate_batch_stride must be a multiple of 4");
+  if (tl) {
+    if (!tl->tail_a || !tl->tail_w) return fail(PXA_ERR_ARG, "null tail_a / tail_w");
+    if (tl->tail_k <= 0 || (tl->tail_k & 7)) return fail(PXA_ERR_ARG, "tail_k must be a positive multiple of 8 (got %d)", tl->tail_k);
+    if (a.operands_mn_major) return fail(PXA_ERR_ARG, "the K-tail does not take operands_mn_major");
+    if (a.epilogue == PXA_EPI_LN_BIAS || a.epilogue == PXA_EPI_LN_BIAS_GELU)
+      return fail(PXA_ERR_ARG, "the K-tail does not take the fused LayerNorm epilogues");
+    if ((reinterpret_cast<uintptr_t>(tl->tail_a) | reinterpret_cast<uintptr_t>(tl->tail_w)) & 15)
+      return fail(PXA_ERR_ALIGN, "tail_a / tail_w must be 16-byte aligned");
+    if ((tl->lda_tail & 7) || (tl->ldw_tail & 7))
+      return fail(PXA_ERR_ALIGN, "lda_tail / ldw_tail must be multiples of 8 (got %d, %d)", tl->lda_tail, tl->ldw_tail);
+    if (tl->lda_tail < tl->tail_k || tl->ldw_tail < tl->tail_k) return fail(PXA_ERR_ARG, "lda_tail / ldw_tail < tail_k");
+  }
   PXA_REQUIRE_SM90();
   int bn = a.block_n;
   if (bn == 0) bn = (a.N % 192 == 0) ? 192 : ((a.N % 256 == 0) ? 256 : (a.N >= 192 ? 192 : 128));
@@ -632,8 +686,18 @@ int gemm_bf16_rows(const PxaGemmArgs* args, int row_base, void* stream) {
     return fail(PXA_ERR_ARG, "the fused LayerNorm-modulate needs rows_per_batch >= %d (a tile may span two samples at most)", kBM);
   if (a.res_epilogue < 0 || a.res_epilogue > 2) return fail(PXA_ERR_ARG, "res_epilogue must be 0, 1 or 2");
   if (bn == 256 && a.out_dtype == PXA_DTYPE_F32) bn = 128;   // fp32 output tiles run at 128 columns (GemmCfg)
+  // the tail instantiations spill at BN 256 and, with fp32 output, at BN 192: they run at 192 and 128 instead
+  if (tl && bn == 256) bn = 192;
+  if (tl && bn == 192 && a.out_dtype == PXA_DTYPE_F32) bn = 128;
   if (a.row_stats_out && (a.N + bn - 1) / bn > PXA_LN_STAT_PARTS)
     return fail(PXA_ERR_ARG, "row_stats_out: N / block_n = %d column tiles exceed PXA_LN_STAT_PARTS", (a.N + bn - 1) / bn);
+  if (tl) {
+    switch (bn) {
+      case 128: return dispatch_epi<128, true>(a, s, tl);
+      case 192: return dispatch_epi<192, true>(a, s, tl);
+      default: return fail(PXA_ERR_ARG, "block_n must be 0, 128, 192 or 256 (got %d)", bn);
+    }
+  }
   switch (bn) {
     case 128: return dispatch_epi<128>(a, s);
     case 192: return dispatch_epi<192>(a, s);
@@ -641,6 +705,13 @@ int gemm_bf16_rows(const PxaGemmArgs* args, int row_base, void* stream) {
     default: return fail(PXA_ERR_ARG, "block_n must be 0, 128, 192 or 256 (got %d)", bn);
   }
 }
+
+int gemm_bf16_rows(const PxaGemmArgs* args, int row_base, void* stream) { return gemm_impl(args, row_base, nullptr, stream); }
 }  // namespace pxa
 
 extern "C" int pxa_gemm_bf16(const PxaGemmArgs* args, void* stream) { return pxa::gemm_bf16_rows(args, 0, stream); }
+
+extern "C" int pxa_gemm_lora_bf16(const PxaGemmArgs* args, const PxaGemmTail* tail, void* stream) {
+  if (!tail) return pxa::fail(PXA_ERR_ARG, "null tail");
+  return pxa::gemm_impl(args, 0, tail, stream);
+}

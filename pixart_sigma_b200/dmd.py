@@ -28,12 +28,18 @@ from . import lib
 from .lcm import FlatEMA, LCMScheduler, _ConsistencyLoss, _dup, _inference_copy, _upload
 from .sampler import _capture, _denoiser_key, _denoiser_params, _step_input
 
-__all__ = ["ddpm_alphas_cumprod", "ema_decay", "dmd_draws", "null_caption", "DMDSampler", "DMDDistiller"]
+__all__ = ["ddpm_alphas_cumprod", "ddpm_add_noise", "ema_decay", "dmd_draws", "null_caption", "DMDSampler", "DMDDistiller"]
 
 
 def ddpm_alphas_cumprod(num_train_timesteps: int = 1000) -> torch.Tensor:
     """float32 cumprod(1 - linspace(1e-4, 0.02, T)), as diffusers' `DDPMScheduler` and `LCMScheduler` compute it."""
     return LCMScheduler(num_train_timesteps=num_train_timesteps).alphas_cumprod
+
+
+def ddpm_add_noise(alphas_cumprod: torch.Tensor, x: torch.Tensor, noise: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
+    """`DDPMScheduler.add_noise` on a float32 alphas_cumprod table (on x's device): sqrt(a_t) x + sqrt(1 - a_t) noise."""
+    a = alphas_cumprod[t]
+    return (a ** 0.5).view(-1, 1, 1, 1) * x + ((1 - a) ** 0.5).view(-1, 1, 1, 1) * noise
 
 
 def ema_decay(update: int, max_decay: float = 0.9999) -> float:
@@ -262,8 +268,7 @@ class DMDDistiller:
 
     def add_noise(self, x: torch.Tensor, noise: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
         """`DDPMScheduler.add_noise` (float32 alphas_cumprod): sqrt(a_t) x + sqrt(1 - a_t) noise."""
-        a = self.ac[t]
-        return (a ** 0.5).view(-1, 1, 1, 1) * x + ((1 - a) ** 0.5).view(-1, 1, 1, 1) * noise
+        return ddpm_add_noise(self.ac, x, noise, t)
 
     def _workspace(self, b: int):
         if b not in self._ws:

@@ -40,6 +40,11 @@ class GemmArgs(C.Structure):
                 ("reverse_tiles", C.c_int32)]
 
 
+class GemmTail(C.Structure):
+    _fields_ = [("tail_a", C.c_void_p), ("tail_w", C.c_void_p), ("tail_k", C.c_int32), ("lda_tail", C.c_int32),
+                ("ldw_tail", C.c_int32)]
+
+
 class LnPrepareArgs(C.Structure):
     _fields_ = [("x", C.c_void_p), ("a_out", C.c_void_p), ("stats_out", C.c_void_p), ("scale", C.c_void_p),
                 ("mod_batch_stride", C.c_int64), ("rows_per_batch", C.c_int32), ("M", C.c_int32), ("C", C.c_int32),
@@ -230,7 +235,7 @@ EXPORTS = ("pxa_transpose_bf16", "pxa_gelu_tanh_bf16", "pxa_gate_residual_fwd", 
            "pxa_rmsnorm_bf16", "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step",
            "pxa_grad_clip_flat", "pxa_came_workspace_bytes", "pxa_came_flat",
            "pxa_lcm_step", "pxa_lcm_teacher_target", "pxa_lcm_consistency_loss", "pxa_ema_flat",
-           "pxa_dmd_loss")
+           "pxa_dmd_loss", "pxa_gemm_lora_bf16")
 
 _lib = None
 
@@ -263,6 +268,8 @@ def load() -> C.CDLL:
             fn = getattr(lib, name)
             fn.restype = C.c_int
             fn.argtypes = [C.POINTER(struct), C.c_void_p]
+        lib.pxa_gemm_lora_bf16.restype = C.c_int
+        lib.pxa_gemm_lora_bf16.argtypes = [C.POINTER(GemmArgs), C.POINTER(GemmTail), C.c_void_p]
         lib.pxa_came_workspace_bytes.restype = C.c_int
         lib.pxa_came_workspace_bytes.argtypes = [C.POINTER(CameArgs), C.POINTER(CameParam), C.POINTER(C.c_int64)]
         lib.pxa_layernorm_affine_bf16.restype = C.c_int
@@ -320,8 +327,12 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: to
          row_stats_out: Optional[torch.Tensor] = None, ln_stats: Optional[torch.Tensor] = None,
          ln_u: Optional[torch.Tensor] = None, ln_v: Optional[torch.Tensor] = None, ln_uv_batch_stride: int = 0,
          ln_dim: int = 0, ln_eps: float = 1e-6, res_epilogue: int = 0, epi_warps: int = 0,
-         reverse_tiles: bool = False) -> torch.Tensor:
+         reverse_tiles: bool = False, tail_a: Optional[torch.Tensor] = None,
+         tail_w: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out = epilogue(a @ w.T + bias). a (M,K) bf16, w (N,K) bf16 (nn.Linear layout), both K-contiguous.
+
+    K-tail (pxa_gemm_lora_bf16): with tail_a (M, T) and tail_w (N, T), bf16 K-contiguous, T a multiple of 8, the epilogue is
+    applied to a @ w.T + tail_a @ tail_w.T -- a LoRA up-projection u (s B)^T added before bias / GELU / gated residual.
 
     Fused LayerNorm-modulate (include/pixart_sm100.h, PXA_EPI_LN_BIAS): the fp32 residual epilogue can emit the scaled bf16
     copy `out_aux = out * aux_scale[b]` and the per-row partial sums `row_stats_out` (M, 8, 2); the EPI_LN_* epilogues
@@ -352,7 +363,15 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: to
                     row_stats_out=_ptr(row_stats_out), ln_stats=_ptr(ln_stats), ln_u=_ptr(ln_u), ln_v=_ptr(ln_v),
                     ln_uv_batch_stride=ln_uv_batch_stride, ln_dim=ln_dim, ln_eps=ln_eps, res_epilogue=res_epilogue,
                     epi_warps=epi_warps, reverse_tiles=int(reverse_tiles))
-    _check(load().pxa_gemm_bf16(C.byref(args), _stream()), "pxa_gemm_bf16")
+    if tail_a is None and tail_w is None:
+        _check(load().pxa_gemm_bf16(C.byref(args), _stream()), "pxa_gemm_bf16")
+        return out
+    assert tail_a is not None and tail_w is not None and tail_a.dtype == tail_w.dtype == torch.bfloat16
+    assert tail_a.dim() == 2 and tail_w.dim() == 2 and tail_a.stride(1) == 1 and tail_w.stride(1) == 1
+    T = tail_a.shape[1]
+    assert tail_a.shape[0] == M and tail_w.shape == (N, T)
+    tail = GemmTail(tail_a=_ptr(tail_a), tail_w=_ptr(tail_w), tail_k=T, lda_tail=tail_a.stride(0), ldw_tail=tail_w.stride(0))
+    _check(load().pxa_gemm_lora_bf16(C.byref(args), C.byref(tail), _stream()), "pxa_gemm_lora_bf16")
     return out
 
 

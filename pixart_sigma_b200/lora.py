@@ -14,7 +14,13 @@ peft's per-projection tensors.
     merge_lora(model)          W <- round(W + s B A) computed in fp32; every sampler and GraphedForward then runs unchanged
     unmerge_lora(model)        restore the replaced weights bit for bit
 
-A forward of a model whose adapters are attached but not merged raises instead of silently ignoring them.
+Training: a forward of a CUDA model with an unmerged adapter, with autograd recording, applies the adapter on the kernels
+(`pixart_sigma_b200.autograd`): the down-projection u = x A^T runs as a skinny GEMM and the up-projection s u B^T as a K-tail
+of the projection's own GEMM (`pxa_gemm_lora_bf16`), so that every epilogue sees the sum.  `prepare_operands` builds the bf16
+operands those GEMMs read from the fp32 parameters at the start of each training forward.  The projections that run in fp32
+torch (patch embedding, timestep / size embedders, t_block, final layer) apply their adapters in fp32 torch
+(`linear_fp32`, `conv_fp32`).  Any other forward of a model with an unmerged adapter (no_grad, CPU, a captured
+GraphedForward) raises instead of silently ignoring it.
 """
 from __future__ import annotations
 
@@ -136,6 +142,7 @@ def inject_lora(model: nn.Module, r: int, use_rslora: bool = False, target_modul
         mod.lora_A = nn.Parameter(A.to(w.device))
         mod.lora_B = nn.Parameter(torch.zeros(G, w.shape[0] // G, r, device=w.device))
         mod.__dict__["_lora_names"] = list(groups)
+        mod.__dict__["_lora_scale"] = _scale(r, lora_alpha, use_rslora)
         names += groups
     model.__dict__["_lora"] = {"r": r, "alpha": lora_alpha, "use_rslora": use_rslora, "scale": _scale(r, lora_alpha, use_rslora),
                                "targets": targets, "merged": False}
@@ -279,3 +286,87 @@ def unmerge_lora(model: nn.Module) -> None:
         for _, mod in _adapted(model):
             mod.weight.copy_(mod.__dict__.pop("_lora_saved"))
     st["merged"] = False
+
+
+def active(mod: nn.Module) -> bool:
+    """True when `mod` carries an adapter that is not merged into its weight."""
+    return "_lora_names" in mod.__dict__ and "_lora_saved" not in mod.__dict__
+
+
+class Operands:
+    """bf16 operands of one adapted projection for the kernels, T = G r rounded up to a multiple of 8 (zero columns):
+    a = A [T, K] (u = x A^T), b = s blockdiag(B) [N, T] (forward tail), at = A^T [K, T] (dgrad tail),
+    bt = (s blockdiag(B))^T [T, N] (v = dY s B).  Each is rounded once from fp32."""
+    __slots__ = ("a", "b", "at", "bt", "T", "r", "G", "s")
+
+    def __init__(self, a, b, at, bt, r, G, s):
+        self.a, self.b, self.at, self.bt = a, b, at, bt
+        self.T, self.r, self.G, self.s = a.shape[0], r, G, s
+
+
+def _kernel_modules(model: nn.Module) -> List[nn.Module]:
+    """The adapted projections that run on the GEMM kernels: every block projection and the caption projection."""
+    mods = [model.y_embedder.y_proj.fc1, model.y_embedder.y_proj.fc2]
+    for blk in model.blocks:
+        mods += [blk.attn.qkv, blk.attn.proj, blk.cross_attn.q_linear, blk.cross_attn.kv_linear, blk.cross_attn.proj,
+                 blk.mlp.fc1, blk.mlp.fc2]
+    return [m for m in mods if active(m)]
+
+
+@torch.no_grad()
+def prepare_operands(model: nn.Module) -> None:
+    """(Re)build the bf16 `Operands` of every unmerged adapter on the kernel path from lora_A / lora_B, in place in buffers
+    that persist across calls (so a captured training step sees optimizer updates), with a few batched ops per group of
+    same-shaped projections.  Run at the start of every training forward: optimizers that write `.data` do not bump
+    `_version`, so a cache keyed on it would go stale.  Projections without an active adapter lose their operands."""
+    st = model.__dict__.get("_lora")
+    mods = _kernel_modules(model) if st is not None else []
+    keep = set(map(id, mods))
+    for m in model.modules():
+        if id(m) not in keep:
+            m.__dict__.pop("_pxa_lora", None)
+    if not mods:
+        return
+    r, s = st["r"], st["scale"]
+    cache = model.__dict__.setdefault("_lora_bufs", {})
+    groups: Dict[tuple, List[nn.Module]] = {}
+    for m in mods:
+        groups.setdefault((tuple(m.lora_A.shape), tuple(m.lora_B.shape), m.weight.device), []).append(m)
+    for key, ms in groups.items():
+        (GR, K), (G, Ng, _), dev = key
+        N, T, n = G * Ng, (GR + 7) // 8 * 8, len(ms)
+        bkey = key + (n, tuple(map(id, ms)))
+        bufs = cache.get(bkey)
+        if bufs is None:
+            z = lambda *shape: torch.zeros(shape, dtype=torch.bfloat16, device=dev)
+            bufs = cache[bkey] = (z(n, T, K), z(n, N, T), z(n, K, T), z(n, T, N))
+        a16, b16, at16, bt16 = bufs
+        A = torch.stack([m.lora_A.detach() for m in ms]).float()                  # [n, G r, K]
+        sB = torch.stack([m.lora_B.detach() for m in ms]).float() * s             # [n, G, N/G, r]
+        a16[:, :GR].copy_(A)
+        at16[:, :, :GR].copy_(A.transpose(1, 2))
+        b4, bt4 = b16.view(n, G, Ng, T), bt16.view(n, T, G, Ng)
+        for g in range(G):
+            b4[:, g, :, g * r:(g + 1) * r].copy_(sB[:, g])
+            bt4[:, g * r:(g + 1) * r, g].copy_(sB[:, g].transpose(1, 2))
+        for i, m in enumerate(ms):
+            m.__dict__["_pxa_lora"] = Operands(a16[i], b16[i], at16[i], bt16[i], r, G, s)
+
+
+def linear_fp32(mod: nn.Module, x: torch.Tensor) -> torch.Tensor:
+    """F.linear in fp32 on `mod`'s weight, plus its unmerged adapter: x W^T + b + s (x A^T) B^T."""
+    out = torch.nn.functional.linear(x, mod.weight.float(), None if mod.bias is None else mod.bias.float())
+    if active(mod):
+        out = out + mod._lora_scale * torch.nn.functional.linear(torch.nn.functional.linear(x, mod.lora_A.float()), mod.lora_B[0].float())
+    return out
+
+
+def conv_fp32(mod: nn.Conv2d, x: torch.Tensor) -> torch.Tensor:
+    """The patch-embedding convolution in fp32 plus its unmerged adapter: peft's lora_A is a Conv2d(in, r, k, stride) and
+    lora_B a 1x1 Conv2d(r, out)."""
+    F = torch.nn.functional
+    out = F.conv2d(x, mod.weight.float(), mod.bias.float(), stride=mod.stride)
+    if active(mod):
+        u = F.conv2d(x, mod.lora_A.float(), stride=mod.stride)
+        out = out + mod._lora_scale * F.conv2d(u, mod.lora_B[0].float()[:, :, None, None])
+    return out

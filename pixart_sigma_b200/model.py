@@ -22,6 +22,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import lib
+from . import lora
 from .lora import require_merged as require_lora_merged
 
 __all__ = ["PixArtMS", "PixArtMSBlock", "PixArtMS_XL_2", "MODELS", "build_model", "install_into_reference"]
@@ -110,8 +111,8 @@ class TimestepEmbedder(nn.Module):
 
     def embed_fp32(self, t: torch.Tensor) -> torch.Tensor:
         f = self.timestep_embedding(t, self.frequency_embedding_size)
-        h = F.silu(F.linear(f, self.mlp[0].weight.float(), self.mlp[0].bias.float()))
-        return F.linear(h, self.mlp[2].weight.float(), self.mlp[2].bias.float())
+        h = F.silu(lora.linear_fp32(self.mlp[0], f))                    # (+ an unmerged LoRA adapter's s u B^T, fp32)
+        return lora.linear_fp32(self.mlp[2], h)
 
     def forward(self, t):
         return self.embed_fp32(t).to(self.mlp[0].weight.dtype)
@@ -649,10 +650,13 @@ class PixArtMS(nn.Module):
 
     def forward(self, x, timestep, y, mask=None, data_info=None, **kwargs):
         """x (B, 4, H, W) latents, timestep (B,), y (B, 1, L, 4096) T5 features, mask (n, L) | (B,1,1,L) | None
-        -> (B, 8, H, W)   (PixArtMS.py:165-211)."""
-        require_lora_merged(self)
+        -> (B, 8, H, W)   (PixArtMS.py:165-211).  An unmerged LoRA adapter is applied only by the CUDA training forward
+        (autograd recording); every other forward raises until it is merged."""
         w0 = self.blocks[0].attn.qkv.weight
-        if _wants_grad(self, x, y):
+        train = _wants_grad(self, x, y)
+        if not (train and w0.is_cuda):
+            require_lora_merged(self)
+        if train:
             # the kernels fix their own precisions (bf16 operands, fp32 accumulation / statistics / residual stream); an
             # ambient autocast (accelerate's mixed precision, train.py:369) must not down-cast the fp32 torch glue around them
             with torch.autocast(device_type="cuda", enabled=False):
@@ -722,12 +726,14 @@ class PixArtMS(nn.Module):
         """The same forward recorded for autograd (train_scripts/train.py:189-197): every block op is a
         `torch.autograd.Function` over the sm_90a kernels (autograd.py), blocks marked by `set_grad_checkpoint`
         (diffusion/model/utils.py:28-45) are activation-checkpointed like PixArtMS.py:206.  Parameters may be fp32
-        (mixed precision: the kernels read cached bf16 shadows) or bf16."""
+        (mixed precision: the kernels read cached bf16 shadows) or bf16.  Unmerged LoRA adapters are applied: on the kernel
+        path through the GEMM K-tail (operands rebuilt here from the parameters), on the fp32 torch glue in fp32."""
         from torch.utils.checkpoint import checkpoint
         from . import autograd as ag
         w0 = self.blocks[0].attn.qkv.weight
         if not w0.is_cuda:
             raise RuntimeError(f"PixArtMS: parameters are on {w0.device}; pixart_sigma_b200 has no CPU path")
+        lora.prepare_operands(self)
         dt, dev, C, p = self.dtype, w0.device, self.hidden_size, self.patch_size
         B = x.shape[0]
         x = x.to(device=dev)
@@ -735,8 +741,7 @@ class PixArtMS(nn.Module):
         y = y.to(device=dev)
         self.h, self.w = x.shape[-2] // p, x.shape[-1] // p
         N = self.h * self.w
-        pe = self.x_embedder.proj
-        tok = F.conv2d(x.float(), pe.weight.float(), pe.bias.float(), stride=p).flatten(2).transpose(1, 2)
+        tok = lora.conv_fp32(self.x_embedder.proj, x.float()).flatten(2).transpose(1, 2)
         x32 = (tok + _pos_embed_fp32(C, self.h, self.w, self.pe_interpolation, self.base_size, dev)[None])
         x32 = x32.reshape(B * N, C).contiguous()
         t = self.t_embedder.embed_fp32(timestep)
@@ -744,7 +749,7 @@ class PixArtMS(nn.Module):
             csize = self.csize_embedder.embed_fp32(data_info["img_hw"].to(dev, dt), B)
             ar = self.ar_embedder.embed_fp32(data_info["aspect_ratio"].to(dev, dt), B)
             t = t + torch.cat([csize, ar], dim=1)
-        t0 = F.linear(F.silu(t), self.t_block[1].weight.float(), self.t_block[1].bias.float())
+        t0 = lora.linear_fp32(self.t_block[1], F.silu(t))
         t0 = t0.view(B, 6, C)
 
         ye = self.y_embedder                                                # caption projector (PixArt_blocks.py:400-407)
@@ -774,7 +779,7 @@ class PixArtMS(nn.Module):
         fl = self.final_layer
         fmod = (fl.scale_shift_table.float()[None] + t[:, None]).contiguous()
         xn = ag.LnModulateFn.apply(x32, fmod, 0, 1, N)
-        out = F.linear(xn.float(), fl.linear.weight.float(), fl.linear.bias.float()).view(B, N, -1)
+        out = lora.linear_fp32(fl.linear, xn.float()).view(B, N, -1)
         return self.unpatchify(out).to(self.output_dtype or dt)
 
     def forward_with_dpmsolver(self, x, timestep, y, data_info, **kwargs):

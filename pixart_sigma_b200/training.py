@@ -86,6 +86,38 @@ class IDDPMLoss:
         return terms
 
 
+class DDPMEpsLoss:
+    """The objective of `train_scripts/train_pixart_lora_hf.py`: noise added by diffusers' `DDPMScheduler.add_noise` on its
+    float32 alphas_cumprod (`dmd.ddpm_alphas_cumprod`), model_pred = the first half of the output channels (the epsilon
+    prediction; the learned variance is not trained), and the MSE against the noise.  `training_losses` has IDDPMLoss's
+    contract; its 'loss' is the per-sample mean, so that loss.mean() is the script's `F.mse_loss(..., reduction="mean")`.
+    For LoRA, build the model with class_dropout_prob=0 (the script's diffusers transformer drops no captions) and keep the
+    adapter unmerged while training."""
+
+    def __init__(self, num_train_timesteps: int = 1000, snr_gamma: Optional[float] = None, prediction_type: str = "epsilon"):
+        from .dmd import ddpm_alphas_cumprod
+        if snr_gamma is not None:
+            raise NotImplementedError("snr_gamma loss weighting is not supported")
+        if prediction_type != "epsilon":
+            raise NotImplementedError(f"prediction_type={prediction_type!r} is not supported (only 'epsilon')")
+        self.num_timesteps = num_train_timesteps
+        self.alphas_cumprod = ddpm_alphas_cumprod(num_train_timesteps)
+        self._dev: Dict[str, torch.Tensor] = {}
+
+    def training_losses(self, model, x_start, timestep, model_kwargs: Optional[dict] = None, noise=None) -> Dict[str, torch.Tensor]:
+        from .dmd import ddpm_add_noise
+        if noise is None:
+            noise = torch.randn_like(x_start)
+        key = str(x_start.device)
+        if key not in self._dev:
+            self._dev[key] = self.alphas_cumprod.to(x_start.device)
+        x_t = ddpm_add_noise(self._dev[key], x_start, noise, timestep)
+        out = model(x_t, timestep=timestep, **(model_kwargs or {}))
+        pred = out.chunk(2, 1)[0].float()
+        mse = ((pred - noise.float()) ** 2).flatten(1).mean(1)
+        return {"mse": mse, "loss": mse}
+
+
 def train_step(model, loss_fn: IDDPMLoss, x_start, timestep, y, mask, data_info=None, noise=None, reducer=None,
                loss_scale: float = 1.0, refresh_shadows: bool = True) -> torch.Tensor:
     """One fwd + bwd of `train_scripts/train.py:186-197` (the optimizer step stays the caller's): returns the mean loss
