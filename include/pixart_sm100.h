@@ -49,7 +49,7 @@ uint64_t pxa_launch_count(void);
 #define PXA_EPI_BIAS 0          /* out = acc + bias                                   */
 #define PXA_EPI_BIAS_GELU 1     /* out = gelu_tanh(acc + bias)                        */
 #define PXA_EPI_BIAS_RESIDUAL 2 /* out = residual + gate[row/rows_per_batch, n] * (acc + bias); gate NULL -> 1 */
-/* Training fusions of the MLP (timm Mlp, PixArtMS.py:67,77), used by pixart_sigma_b200.autograd (PXA_FUSED_MLP=0 turns them off). */
+/* Training fusions of the MLP (timm Mlp, PixArtMS.py:67,77), used by the block backward of pixart_sigma_b200.autograd. */
 #define PXA_EPI_BIAS_GELU_AUX 3 /* out = gelu_tanh(acc + bias), out_aux_bf16 = acc + bias (pre-activation kept for the backward) */
 #define PXA_EPI_MUL_DGELU 4     /* out = acc * gelu_tanh'(pre), pre = `residual` as bf16 [M, N] row stride ldo; bias must be NULL  */
 /* adaLN-single modulate FUSED into the projection that follows it (norm1 + t2i_modulate + attn.qkv, PixArtMS.py:75 with

@@ -1,19 +1,22 @@
-"""Training path: the block's ops as `torch.autograd.Function`s whose forward AND backward are sm_90a kernels.
+"""Training path: `torch.autograd.Function`s whose forward AND backward are sm_90a kernels.
 
 The reference trains through torch autograd (`train_scripts/train.py:197 accelerator.backward(loss)`) with per-block
 activation checkpointing (`diffusion/model/utils.py:28-45`, call site `PixArtMS.py:206`).  Here autograd is only the
 tape: every node below calls into libpixart_sm100.so in both directions --
 
+  BlockFn         one whole PixArtMSBlock (PixArtMS.py:71-79) per node, every block kind: qk_norm (PixArt_blocks.py:133-134)
+                  and KV compression (PixArt_blocks.py:97-121, 137-139) included.  Forward: the kernel sequence of
+                  `_block_forward_kernels`; backward: the explicit reverse sequence (flash-attention-2 backward
+                  pxa_flash_attn_d72_bwd_bf16, pxa_gate_residual_bwd, pxa_ln_modulate_bwd, pxa_kv_compress_conv2_ln_bwd and
+                  the Linear backward below per projection).  Activation checkpointing is built in.
+
+and three nodes for the glue around the blocks (caption projector and final layer, `model.PixArtMS._forward_train`):
+
   LinearFn        y = x W^T + b           bwd: dX = dY W (pxa_gemm_bf16 on the cached W^T) and dW += dY^T X (the GEMM's
                                           weight-gradient form: both activations consumed MN-major in their natural
                                           layouts, split-K, fp32 TMA reduce-add epilogue), db by pxa_colsum_bf16
-  LnModulateFn    LN(x)(1+scale)+shift    bwd: pxa_ln_modulate_bwd (dx, d shift, d scale)            PixArtMS.py:75,77
-  LinearGateResidualFn  x + gate*(aW^T+b) one GEMM launch (fp32 residual epilogue, aux = branch); bwd: pxa_gate_residual_bwd
-                                          (d branch, d gate) then the Linear backward            PixArtMS.py:75-77
   GeluFn          gelu_tanh(pre)          bwd: pxa_gelu_tanh_bf16 with dh                            timm Mlp.act
-  SelfAttnFn / CrossAttnFn / AttnKVFn     bwd: pxa_flash_attn_d72_bwd_bf16 (flash-attention-2 recomputation from lse)
-                                                                                                PixArt_blocks.py:52-53,153
-  KvCompressFn    LN(conv2x2s2(k | v))    bwd: pxa_kv_compress_conv2_ln_bwd                       PixArt_blocks.py:97-121
+  LnModulateFn    LN(x)(1+scale)+shift    bwd: pxa_ln_modulate_bwd (dx, d shift, d scale)            PixArt_blocks.py:219
 
 LoRA: a projection with an unmerged adapter (lora.py; operands from `lora.prepare_operands`) adds s u B^T with u = x A^T:
 u is a skinny GEMM (N = T), and the up-projection is a K-tail of the projection's own GEMM (`lib.gemm(tail_a=u,
@@ -31,15 +34,8 @@ from typing import Optional
 
 import torch
 
-import os
-
 from . import lib
 
-# MLP branch as two GEMM launches with the GELU forward / backward inside their epilogues (MlpGateResidualFn), covered by
-# tests/test_training_gpu.py and test_backward_gpu.py.  PXA_FUSED_MLP=0 restores the separate GELU passes.
-_FUSED_MLP = os.environ.get("PXA_FUSED_MLP", "1") == "1"
-# weight / bias gradients are accumulated by the kernels directly into an existing fp32 .grad (PXA_DIRECT_GRAD=0: via autograd)
-_DIRECT_GRAD = os.environ.get("PXA_DIRECT_GRAD", "1") == "1"
 
 def _shadow(mod: torch.nn.Module, kind: str) -> Optional[torch.Tensor]:
     """bf16 copy of `mod.weight` ('w'), its bf16 transpose ('t') or the bf16 bias ('b'), cached ON THE MODULE and
@@ -228,7 +224,7 @@ def _linear_backward(ctx_needs, x, weight, bias, mod, dy, u=None, v=None, lora_n
 def _grad_accumulator(p: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
     """The tensor a backward kernel may accumulate a parameter gradient into directly: the parameter's existing fp32,
     contiguous `.grad` (e.g. its view into a `parallel.GradBucketReducer` bucket).  None -> hand the gradient to autograd."""
-    if p is None or not _DIRECT_GRAD:
+    if p is None:
         return None
     g = p.grad
     if g is None or g.dtype != torch.float32 or not g.is_contiguous() or g.device != p.device or g.shape != p.shape:
@@ -242,98 +238,6 @@ def _grad_landed(p: torch.Tensor) -> None:
     cb = getattr(p, "_pxa_grad_ready", None)
     if cb is not None:
         cb()
-
-
-class LinearGateResidualFn(torch.autograd.Function):
-    """out = x32 + tab[:, i_gate] * (a W^T + b) in ONE GEMM launch (fp32 residual epilogue, PixArtMS.py:75-77): the
-    branch output never makes a separate pass; with a gate it is kept (bf16 aux output of the epilogue) because the
-    gate's gradient is sum_rows dout * branch."""
-
-    @staticmethod
-    def forward(ctx, a, weight, bias, mod, x32, tab, i_gate, rows_per_batch, lora_A=None, lora_B=None):
-        a, x32 = a.contiguous(), x32.contiguous()
-        M, N = a.shape[0], weight.shape[0]
-        out = torch.empty((M, N), dtype=torch.float32, device=a.device)
-        gated = i_gate >= 0
-        y = torch.empty((M, N), dtype=torch.bfloat16, device=a.device) if gated else None
-        u = _lora_u(a, mod)
-        lib.gemm(a, _shadow(mod, "w"), _shadow(mod, "b"), out, epilogue=lib.EPI_BIAS_RESIDUAL, residual=x32,
-                 gate=tab[:, i_gate] if gated else None, gate_batch_stride=tab.stride(0) if gated else 0,
-                 rows_per_batch=rows_per_batch, out_aux=y, aux_is_branch=True, **_tail(u, mod, "b"))
-        ctx.save_for_backward(a, weight, bias, y, tab if gated else None, u)
-        ctx.mod, ctx.idx = mod, (i_gate, rows_per_batch)
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        a, weight, bias, y, tab, u = ctx.saved_tensors
-        i_gate, rpb = ctx.idx
-        dout = dout.contiguous()
-        dy = torch.empty(dout.shape, dtype=torch.bfloat16, device=dout.device)
-        dtab = None
-        if tab is not None:
-            want = ctx.needs_input_grad[5]
-            dg = torch.zeros((tab.shape[0], tab.shape[2]), dtype=torch.float32, device=dout.device) if want else None
-            lib.gate_residual_bwd(dout, y if want else None, tab[:, i_gate], dy, dg, gate_batch_stride=tab.stride(0),
-                                  rows_per_batch=rpb)
-            if want:
-                dtab = torch.zeros_like(tab)
-                dtab[:, i_gate] = dg
-        else:
-            lib.gate_residual_bwd(dout, None, None, dy, None, rows_per_batch=rpb)
-        n = ctx.needs_input_grad
-        da, dw, db, dA, dB = _linear_backward(n[:3], a, weight, bias, ctx.mod, dy, u=u, lora_needs=n[8:10])
-        return da, dw, db, None, dout, dtab, None, None, dA, dB
-
-
-class MlpGateResidualFn(torch.autograd.Function):
-    """The whole MLP branch
-    out = x32 + gate * fc2(gelu(fc1(xn))) in TWO GEMM launches -- fc1 with the GELU epilogue that also keeps the
-    pre-activation (EPI_BIAS_GELU_AUX), fc2 with the gated residual epilogue -- and a backward whose fc2 dgrad GEMM applies
-    gelu'(pre) in its epilogue (EPI_MUL_DGELU): no separate GELU forward / backward passes over the [M, 4C] hidden."""
-
-    @staticmethod
-    def forward(ctx, xn, w1, b1, w2, b2, fc1, fc2, x32, tab, i_gate, rows_per_batch, A1=None, B1=None, A2=None, B2=None):
-        xn, x32 = xn.contiguous(), x32.contiguous()
-        M, Hd, N = xn.shape[0], w1.shape[0], w2.shape[0]
-        bf = dict(dtype=torch.bfloat16, device=xn.device)
-        h, pre = torch.empty((M, Hd), **bf), torch.empty((M, Hd), **bf)
-        u1 = _lora_u(xn, fc1)
-        lib.gemm(xn, _shadow(fc1, "w"), _shadow(fc1, "b"), h, epilogue=lib.EPI_BIAS_GELU_AUX, out_aux=pre,
-                 **_tail(u1, fc1, "b"))
-        out = torch.empty((M, N), dtype=torch.float32, device=xn.device)
-        y = torch.empty((M, N), **bf)
-        u2 = _lora_u(h, fc2)
-        lib.gemm(h, _shadow(fc2, "w"), _shadow(fc2, "b"), out, epilogue=lib.EPI_BIAS_RESIDUAL, residual=x32, gate=tab[:, i_gate],
-                 gate_batch_stride=tab.stride(0), rows_per_batch=rows_per_batch, out_aux=y, aux_is_branch=True,
-                 **_tail(u2, fc2, "b"))
-        ctx.save_for_backward(xn, pre, h, y, tab, w1, b1, w2, b2, u1, u2)
-        ctx.mods, ctx.idx = (fc1, fc2), (i_gate, rows_per_batch)
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        xn, pre, h, y, tab, w1, b1, w2, b2, u1, u2 = ctx.saved_tensors
-        n = ctx.needs_input_grad
-        fc1, fc2 = ctx.mods
-        i_gate, rpb = ctx.idx
-        dout = dout.contiguous()
-        dev = dout.device
-        dy = torch.empty(dout.shape, dtype=torch.bfloat16, device=dev)
-        want = ctx.needs_input_grad[8]
-        dg = torch.zeros((tab.shape[0], tab.shape[2]), dtype=torch.float32, device=dev) if want else None
-        lib.gate_residual_bwd(dout, y if want else None, tab[:, i_gate], dy, dg, gate_batch_stride=tab.stride(0), rows_per_batch=rpb)
-        dtab = None
-        if want:
-            dtab = torch.zeros_like(tab)
-            dtab[:, i_gate] = dg
-        v2 = _lora_v(dy, fc2, u2)
-        _, dw2, db2, dA2, dB2 = _linear_backward((False, n[3], n[4]), h, w2, b2, fc2, dy, u=u2, v=v2, lora_needs=n[13:15])
-        dpre = torch.empty_like(pre)
-        lib.gemm(dy, _shadow(fc2, "t"), None, dpre, epilogue=lib.EPI_MUL_DGELU, residual=pre,     # dh * gelu'(pre) in the epilogue
-                 **_tail(v2, fc2, "at"))
-        dxn, dw1, db1, dA1, dB1 = _linear_backward((True, n[1], n[2]), xn, w1, b1, fc1, dpre, u=u1, lora_needs=n[11:13])
-        return dxn, dw1, db1, dw2, db2, None, None, dout, dtab, None, None, dA1, dB1, dA2, dB2
 
 
 class LnModulateFn(torch.autograd.Function):
@@ -387,273 +291,84 @@ def _fp32_p(attn) -> bool:
     return bool(getattr(attn, "fp32_attention", False))
 
 
-class SelfAttnFn(torch.autograd.Function):
-    """o (B*N, C) = attention over the q/k/v slices of the qkv GEMM output (B*N, 3C) (PixArt_blocks.py:130-153)."""
-
-    @staticmethod
-    def forward(ctx, qkv, B, H, N, scale, keep, fp32_p=False):
-        qkv = qkv.contiguous()
-        M, C3 = qkv.shape
-        C = C3 // 3
-        D = C // H
-        q3 = qkv.view(M, 3, H, D)
-        hit = keep.pop("self", None) if keep is not None and keep.get("replay") else None
-        if hit is not None:                           # recomputation of a checkpointed block: (o, lse) were kept
-            o, lse = hit
-        else:
-            o = torch.empty((M, C), dtype=torch.bfloat16, device=qkv.device)
-            lse = torch.empty((B, H, N), dtype=torch.float32, device=qkv.device)
-            st = (3 * C, D)
-            lib.flash_attn(q3[:, 0], q3[:, 1], q3[:, 2], o, B=B, H=H, Nq=N, Nk=N, kv_rows=M, q_strides=st, k_strides=st,
-                           v_strides=st, scale=scale, lse=lse, fp32_p=fp32_p)
-            if keep is not None and not keep.get("replay"):
-                keep["self"] = (o, lse)
-        ctx.save_for_backward(qkv, o, lse)
-        ctx.geom = (B, H, N, scale)
-        return o
-
-    @staticmethod
-    def backward(ctx, d_o):
-        qkv, o, lse = ctx.saved_tensors
-        B, H, N, scale = ctx.geom
-        M, C3 = qkv.shape
-        C = C3 // 3
-        D = C // H
-        q3 = qkv.view(M, 3, H, D)
-        dqkv = torch.empty_like(qkv)
-        d3 = dqkv.view(M, 3, H, D)
-        st = (3 * C, D)
-        lib.flash_attn_bwd(q3[:, 0], q3[:, 1], q3[:, 2], o, d_o.contiguous(), lse, d3[:, 0], d3[:, 1], d3[:, 2], B=B, H=H,
-                           Nq=N, Nk=N, kv_rows=M, q_strides=st, k_strides=st, v_strides=st, dq_strides=st, dk_strides=st,
-                           dv_strides=st, scale=scale)
-        return dqkv, None, None, None, None, None, None
-
-
-class QkNormFn(torch.autograd.Function):
-    """qkv (M, 3C) bf16 with q_norm / k_norm (nn.LayerNorm(C), affine) applied to the q and k slices (PixArt_blocks.py:133-134).
-    Backward: the LayerNorm-modulate backward kernel with one "sample" spanning all rows, scale = weight - 1, shift = bias --
-    its dscale / dshift column sums are the gradients of weight / bias."""
-
-    @staticmethod
-    def forward(ctx, qkv, qw, qb, kw, kb, eps):
-        out = qkv.clone()
-        C = qkv.shape[1] // 3
-        bf = torch.bfloat16
-        lib.layernorm_affine_(out[:, :C], qw.to(bf), qb.to(bf), eps=eps)
-        lib.layernorm_affine_(out[:, C:2 * C], kw.to(bf), kb.to(bf), eps=eps)
-        ctx.save_for_backward(qkv, qw, kw)
-        ctx.eps = eps
-        return out
-
-    @staticmethod
-    def backward(ctx, d_out):
-        qkv, qw, kw = ctx.saved_tensors
-        M, C3 = qkv.shape
-        C = C3 // 3
-        dqkv = d_out.clone()
-        grads = []
-        for i, w in enumerate((qw, kw)):
-            x32 = qkv[:, i * C:(i + 1) * C].float().contiguous()
-            dx = torch.empty_like(x32)
-            dsh = torch.zeros((1, C), dtype=torch.float32, device=qkv.device)
-            dsc = torch.zeros((1, C), dtype=torch.float32, device=qkv.device)
-            lib.ln_modulate_bwd(x32, d_out[:, i * C:(i + 1) * C].contiguous(), (w.float() - 1.0).view(1, C).contiguous(), dx, dsh, dsc,
-                                mod_batch_stride=C, rows_per_batch=M, eps=ctx.eps)
-            dqkv[:, i * C:(i + 1) * C] = dx
-            grads += [dsc.view(C).to(w.dtype), dsh.view(C).to(w.dtype)]
-        return dqkv, grads[0], grads[1], grads[2], grads[3], None
-
-
-def _qk_norm(a, qkv: torch.Tensor) -> torch.Tensor:
-    if isinstance(a.q_norm, torch.nn.Identity):
-        return qkv
-    return QkNormFn.apply(qkv, a.q_norm.weight, a.q_norm.bias, a.k_norm.weight, a.k_norm.bias, a.q_norm.eps)
-
-
-class KvCompressFn(torch.autograd.Function):
-    """(kc, vc) = LN(conv2x2s2(k)), LN(conv2x2s2(v)) on the k / v slices of the qkv GEMM output (PixArt_blocks.py:97-121,
-    'conv' sampling, scale factor 2).  sr = the depthwise Conv2d, norm = the LayerNorm (owners of the bf16 shadows)."""
-
-    @staticmethod
-    def forward(ctx, qkv, sr_w, sr_b, ln_w, ln_b, sr, norm, B, Hh, Ww):
-        qkv = qkv.contiguous()
-        M, C3 = qkv.shape
-        C = C3 // 3
-        n_out = (Hh // 2) * (Ww // 2)
-        kc = torch.empty((B * n_out, C), dtype=torch.bfloat16, device=qkv.device)
-        vc = torch.empty_like(kc)
-        lib.kv_compress(qkv[:, C:2 * C], qkv[:, 2 * C:], kc.view(B, n_out, C), vc.view(B, n_out, C), _shadow(sr, "w"), _shadow(sr, "b"),
-                        _shadow(norm, "w"), _shadow(norm, "b"), B=B, H=Hh, W=Ww, ld_in=C3, eps=norm.eps)
-        ctx.save_for_backward(qkv, sr_w, sr_b, ln_w, ln_b)
-        ctx.mods, ctx.geom = (sr, norm), (B, Hh, Ww)
-        return kc, vc
-
-    @staticmethod
-    def backward(ctx, dkc, dvc):
-        qkv, sr_w, sr_b, ln_w, ln_b = ctx.saved_tensors
-        sr, norm = ctx.mods
-        B, Hh, Ww = ctx.geom
-        M, C3 = qkv.shape
-        C = C3 // 3
-        dqkv = torch.zeros_like(qkv)                    # the q slice gets its gradient from the attention node
-        f32 = dict(dtype=torch.float32, device=qkv.device)
-        g_w, g_b = torch.zeros(sr_w.shape, **f32), torch.zeros(sr_b.shape, **f32)
-        g_lw, g_lb = torch.zeros(ln_w.shape, **f32), torch.zeros(ln_b.shape, **f32)
-        lib.kv_compress_bwd(qkv[:, C:2 * C], qkv[:, 2 * C:], dkc.contiguous(), dvc.contiguous(), dqkv[:, C:2 * C], dqkv[:, 2 * C:],
-                            _shadow(sr, "w"), _shadow(sr, "b"), _shadow(norm, "w"), g_w, g_b, g_lw, g_lb, B=B, H=Hh, W=Ww,
-                            ld_in=C3, ld_din=C3, eps=norm.eps)
-        return (dqkv, g_w.to(sr_w.dtype), g_b.to(sr_b.dtype), g_lw.to(ln_w.dtype), g_lb.to(ln_b.dtype), None, None, None, None, None)
-
-
-class AttnKVFn(torch.autograd.Function):
-    """o = attention of the q slice of qkv (B*N, 3C) over separate, already compressed keys / values (B*Nk, C)
-    (KV-compressed self-attention, PixArt_blocks.py:137-153)."""
-
-    @staticmethod
-    def forward(ctx, qkv, kc, vc, B, H, N, Nk, scale, fp32_p=False):
-        qkv, kc, vc = qkv.contiguous(), kc.contiguous(), vc.contiguous()
-        M, C3 = qkv.shape
-        C = C3 // 3
-        D = C // H
-        o = torch.empty((M, C), dtype=torch.bfloat16, device=qkv.device)
-        lse = torch.empty((B, H, N), dtype=torch.float32, device=qkv.device)
-        lib.flash_attn(qkv[:, :C], kc, vc, o, B=B, H=H, Nq=N, Nk=Nk, kv_rows=B * Nk, q_strides=(C3, D), k_strides=(C, D),
-                       v_strides=(C, D), scale=scale, lse=lse, fp32_p=fp32_p)
-        ctx.save_for_backward(qkv, kc, vc, o, lse)
-        ctx.geom = (B, H, N, Nk, scale)
-        return o
-
-    @staticmethod
-    def backward(ctx, d_o):
-        qkv, kc, vc, o, lse = ctx.saved_tensors
-        B, H, N, Nk, scale = ctx.geom
-        M, C3 = qkv.shape
-        C = C3 // 3
-        D = C // H
-        dqkv = torch.zeros_like(qkv)                    # k / v slices: gradient arrives through the compression node
-        dkc, dvc = torch.empty_like(kc), torch.empty_like(vc)
-        lib.flash_attn_bwd(qkv[:, :C], kc, vc, o, d_o.contiguous(), lse, dqkv[:, :C], dkc, dvc, B=B, H=H, Nq=N, Nk=Nk,
-                           kv_rows=B * Nk, q_strides=(C3, D), k_strides=(C, D), v_strides=(C, D), dq_strides=(C3, D),
-                           dk_strides=(C, D), dv_strides=(C, D), scale=scale)
-        return dqkv, dkc, dvc, None, None, None, None, None, None
-
-
-class CrossAttnFn(torch.autograd.Function):
-    """o (B*N, C) = var-len attention of q (B*N, C) over the caption keys kv (rows, 2C) (PixArt_blocks.py:43-58)."""
-
-    @staticmethod
-    def forward(ctx, q, kv, kv_len, kv_off, B, H, N, max_keys, scale, keep):
-        q, kv = q.contiguous(), kv.contiguous()
-        M, C = q.shape
-        D = C // H
-        kv4 = kv.view(-1, 2, H, D)
-        hit = keep.pop("cross", None) if keep is not None and keep.get("replay") else None
-        if hit is not None:
-            o, lse = hit
-        else:
-            o = torch.empty((M, C), dtype=torch.bfloat16, device=q.device)
-            lse = torch.empty((B, H, N), dtype=torch.float32, device=q.device)
-            lib.flash_attn(q, kv4[:, 0], kv4[:, 1], o, B=B, H=H, Nq=N, Nk=max_keys, kv_rows=kv.shape[0], kv_len=kv_len,
-                           kv_off=kv_off, q_strides=(C, D), k_strides=(2 * C, D), v_strides=(2 * C, D), scale=scale, lse=lse)
-            if keep is not None and not keep.get("replay"):
-                keep["cross"] = (o, lse)
-        ctx.save_for_backward(q, kv, o, lse, kv_len, kv_off)
-        ctx.geom = (B, H, N, max_keys, scale)
-        return o
-
-    @staticmethod
-    def backward(ctx, d_o):
-        q, kv, o, lse, kv_len, kv_off = ctx.saved_tensors
-        B, H, N, max_keys, scale = ctx.geom
-        M, C = q.shape
-        D = C // H
-        kv4 = kv.view(-1, 2, H, D)
-        dq = torch.empty_like(q)
-        dkv = torch.zeros_like(kv)                    # rows of keys >= kv_len[b] (padding) get no gradient
-        d4 = dkv.view(-1, 2, H, D)
-        lib.flash_attn_bwd(q, kv4[:, 0], kv4[:, 1], o, d_o.contiguous(), lse, dq, d4[:, 0], d4[:, 1], B=B, H=H, Nq=N,
-                           Nk=max_keys, kv_rows=kv.shape[0], kv_len=kv_len, kv_off=kv_off, q_strides=(C, D),
-                           k_strides=(2 * C, D), v_strides=(2 * C, D), dq_strides=(C, D), dk_strides=(2 * C, D),
-                           dv_strides=(2 * C, D), scale=scale)
-        return dq, dkv, None, None, None, None, None, None, None, None
-
-
 def linear(x: torch.Tensor, mod: torch.nn.Linear) -> torch.Tensor:
     return LinearFn.apply(x, mod.weight, mod.bias, mod, *_lora_params(mod))
 
 
-def _compressed_self_attention(a, qkv: torch.Tensor, B: int, H: int, N: int, HW) -> torch.Tensor:
-    """Self-attention over compressed keys / values (PixArt_blocks.py:97-121): 'conv' (scale factor 2) runs the fused
-    conv + LN kernel and its backward; the parameter-free samplings are strided picks (pure data movement, torch)."""
-    C = qkv.shape[1] // 3
-    Hh, Ww = HW
-    sr = a.sr_ratio
-    if a.sampling == "conv":
-        if sr != 2:
-            raise NotImplementedError("conv KV compression kernel is specialised for scale_factor 2")
-        kc, vc = KvCompressFn.apply(qkv, a.sr.weight, a.sr.bias, a.norm.weight, a.norm.bias, a.sr, a.norm, B, Hh, Ww)
-    elif a.sampling == "uniform_every":
-        kc, vc = (qkv[:, i * C:(i + 1) * C].reshape(B, N, C)[:, ::sr].reshape(-1, C) for i in (1, 2))
-    elif a.sampling in ("uniform", "ave"):
-        kc, vc = (qkv[:, i * C:(i + 1) * C].reshape(B, Hh, Ww, C)[:, ::sr, ::sr].reshape(-1, C) for i in (1, 2))
-    else:
-        raise ValueError(a.sampling)
-    return AttnKVFn.apply(qkv, kc, vc, B, H, N, kc.shape[0] // B, a.scale, _fp32_p(a))
-
-
-def block_forward_train(blk, x32: torch.Tensor, cond: torch.Tensor, kv_len: Optional[torch.Tensor],
-                        kv_off: Optional[torch.Tensor], max_keys: int, mod: torch.Tensor, B: int, N: int,
-                        keep: Optional[dict] = None, HW=None) -> torch.Tensor:
-    """One PixArtMSBlock (PixArtMS.py:71-79) on the differentiable kernel ops; same arguments as `run_kernels`, but
-    out of place (returns the new fp32 residual stream) so autograd / activation checkpointing can replay it.
-    `keep`: per-call dict used with activation checkpointing -- the first pass stores the two attention outputs and
-    their softmax statistics in it (76 MB per block at 4 x 4096 tokens), the recomputation pass (keep["replay"] set)
-    takes them back instead of re-running the attention kernels."""
-    a, ca, mlp = blk.attn, blk.cross_attn, blk.mlp
-    H = a.num_heads
-    if HW is None:
-        HW = (int(N ** 0.5),) * 2
-    mod = mod.contiguous()
-    # (1) x += gate_msa * proj(attn(LN(x) * (1 + scale_msa) + shift_msa))                         PixArtMS.py:75
-    xn = LnModulateFn.apply(x32, mod, 0, 1, N)
-    if a.sr_ratio > 1:                                                       # KV token compression, PixArt_blocks.py:137-139
-        ao = _compressed_self_attention(a, _qk_norm(a, linear(xn, a.qkv)), B, H, N, HW)
-    else:
-        ao = SelfAttnFn.apply(_qk_norm(a, linear(xn, a.qkv)), B, H, N, a.scale, keep, _fp32_p(a))
-    x32 = LinearGateResidualFn.apply(ao, a.proj.weight, a.proj.bias, a.proj, x32, mod, 2, N, *_lora_params(a.proj))
-    # (2) x += proj(cross_attn(x, cond))                                                          PixArtMS.py:76
-    qx = linear(x32.to(torch.bfloat16), ca.q_linear)
-    kv = linear(cond, ca.kv_linear)
-    ao = CrossAttnFn.apply(qx, kv, kv_len, kv_off, B, H, N, max_keys, ca.head_dim ** -0.5, keep)
-    x32 = LinearGateResidualFn.apply(ao, ca.proj.weight, ca.proj.bias, ca.proj, x32, mod, -1, N, *_lora_params(ca.proj))
-    # (3) x += gate_mlp * fc2(gelu_tanh(fc1(LN(x) * (1 + scale_mlp) + shift_mlp)))               PixArtMS.py:77
-    xn = LnModulateFn.apply(x32, mod, 3, 4, N)
-    if _FUSED_MLP:                                    # experimental, see MlpGateResidualFn
-        x32 = MlpGateResidualFn.apply(xn, mlp.fc1.weight, mlp.fc1.bias, mlp.fc2.weight, mlp.fc2.bias, mlp.fc1, mlp.fc2, x32, mod, 5, N,
-                                      *_lora_params(mlp.fc1), *_lora_params(mlp.fc2))
-    else:
-        h = GeluFn.apply(linear(xn, mlp.fc1))
-        x32 = LinearGateResidualFn.apply(h, mlp.fc2.weight, mlp.fc2.bias, mlp.fc2, x32, mod, 5, N, *_lora_params(mlp.fc2))
-    if keep is not None:
-        keep["replay"] = True            # the next call with this dict is the recomputation
-    return x32
-
-
 # ------------------------------------------------------------------------------------------------- the whole block as ONE node
-_BLOCK_FN = os.environ.get("PXA_BLOCK_FN", "1") == "1"
-
-
 _TAGS = ("qkv", "proj", "q", "kv", "cproj", "fc1", "fc2")
 
 
+def _norms_qk(a) -> bool:
+    return not isinstance(a.q_norm, torch.nn.Identity)
+
+
 def _block_params(blk):
-    """The block's projections in _TAGS order and, per projection, (weight, bias, lora_A, lora_B) (None: no adapter)."""
+    """The block's parameters as BlockFn inputs: per projection in _TAGS order (weight, bias, lora_A, lora_B) (None: no
+    adapter), then (weight, bias) of q_norm and k_norm (qk_norm) and of sr and norm (conv KV compression) where the block
+    has them.  A plain block has 28."""
     a, ca, mlp = blk.attn, blk.cross_attn, blk.mlp
     mods = (a.qkv, a.proj, ca.q_linear, ca.kv_linear, ca.proj, mlp.fc1, mlp.fc2)
-    return mods, tuple(t for m in mods for t in (m.weight, m.bias, *_lora_params(m)))
+    extra = ((a.q_norm, a.k_norm) if _norms_qk(a) else ()) + ((a.sr, a.norm) if a.sr_ratio > 1 and a.sampling == "conv" else ())
+    return tuple(t for m in mods for t in (m.weight, m.bias, *_lora_params(m))) + tuple(t for m in extra for t in (m.weight, m.bias))
 
 
-def _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, kept=None):
+def _kv_pick(a, x, B, N, HW):
+    """The rows of x (B*N, C) that a parameter-free KV compression keeps (PixArt_blocks.py:97-121), as a strided view."""
+    sr = a.sr_ratio
+    if a.sampling == "uniform_every":
+        return x.view(B, N, -1)[:, ::sr]
+    if a.sampling in ("uniform", "ave"):           # the reference's 'ave' is nearest-neighbour = the same strided pick
+        return x.view(B, HW[0], HW[1], -1)[:, ::sr, ::sr]
+    raise ValueError(a.sampling)
+
+
+def _compress_kv(a, qkv, B, N, HW):
+    """(kc, vc) (B*Nk, C): the compressed keys / values of the qkv GEMM output.  'conv' (scale factor 2) runs the fused
+    conv + LN kernel; the parameter-free samplings are strided picks (pure data movement, torch)."""
+    C3 = qkv.shape[1]
+    C = C3 // 3
+    k, v = qkv[:, C:2 * C], qkv[:, 2 * C:]
+    if a.sampling != "conv":
+        return tuple(_kv_pick(a, x, B, N, HW).contiguous().view(-1, C) for x in (k, v))
+    if a.sr_ratio != 2:
+        raise NotImplementedError("conv KV compression kernel is specialised for scale_factor 2")
+    Hh, Ww = HW
+    n_out = (Hh // 2) * (Ww // 2)
+    kc = torch.empty((B * n_out, C), dtype=torch.bfloat16, device=qkv.device)
+    vc = torch.empty_like(kc)
+    lib.kv_compress(k, v, kc.view(B, n_out, C), vc.view(B, n_out, C), _shadow(a.sr, "w"), _shadow(a.sr, "b"),
+                    _shadow(a.norm, "w"), _shadow(a.norm, "b"), B=B, H=Hh, W=Ww, ld_in=C3, eps=a.norm.eps)
+    return kc, vc
+
+
+def _compress_kv_bwd(a, qkv, dkc, dvc, dqkv, B, N, HW):
+    """Backward of `_compress_kv`: the gradients of kc / vc into the k / v slices of dqkv (zero-filled by the caller).  Returns
+    the fp32 gradients of sr.weight, sr.bias, norm.weight, norm.bias ('conv'), else []."""
+    C3 = qkv.shape[1]
+    C = C3 // 3
+    if a.sampling != "conv":
+        for d, dx in ((dkc, dqkv[:, C:2 * C]), (dvc, dqkv[:, 2 * C:])):
+            pick = _kv_pick(a, dx, B, N, HW)
+            pick.copy_(d.view(pick.shape))
+        return []
+    g = [torch.zeros(p.shape, dtype=torch.float32, device=qkv.device) for p in (a.sr.weight, a.sr.bias, a.norm.weight, a.norm.bias)]
+    lib.kv_compress_bwd(qkv[:, C:2 * C], qkv[:, 2 * C:], dkc, dvc, dqkv[:, C:2 * C], dqkv[:, 2 * C:], _shadow(a.sr, "w"),
+                        _shadow(a.sr, "b"), _shadow(a.norm, "w"), *g, B=B, H=HW[0], W=HW[1], ld_in=C3, ld_din=C3, eps=a.norm.eps)
+    return g
+
+
+def _self_kv(t, B, H, N):
+    """(k, v, their (row, head) strides, Nk) of the self-attention: the k / v slices of qkv, or the compressed kc / vc."""
+    M, C3 = t["qkv"].shape
+    D = C3 // 3 // H
+    if "kc" in t:
+        return t["kc"], t["vc"], (C3 // 3, D), t["kc"].shape[0] // B
+    q3 = t["qkv"].view(M, 3, H, D)
+    return q3[:, 1], q3[:, 2], (C3, D), N
+
+
+def _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, HW, kept=None):
     """The block's forward on the kernels, out of place, returning every intermediate the backward reads.  `kept` = the two
     attention outputs + softmax statistics of an earlier pass and its adapter down-projections u_<tag> (activation
     checkpointing: they are not recomputed)."""
@@ -673,12 +388,19 @@ def _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, 
 
     t["xn1"] = lib.ln_modulate(x32, mod[:, 0], mod[:, 1], torch.empty((M, C), **bf), mod_batch_stride=ms, rows_per_batch=N)
     t["qkv"] = gemm("qkv", t["xn1"], a.qkv, torch.empty((M, 3 * C), **bf))
+    if _norms_qk(a):                                  # q_norm / k_norm, PixArt_blocks.py:133-134; the backward reads qkv_pre
+        t["qkv_pre"], t["qkv"] = t["qkv"], t["qkv"].clone()
+        for i, ln in enumerate((a.q_norm, a.k_norm)):
+            lib.layernorm_affine_(t["qkv"][:, i * C:(i + 1) * C], _shadow(ln, "w"), _shadow(ln, "b"), eps=ln.eps)
+    if a.sr_ratio > 1:                                # KV token compression, PixArt_blocks.py:137-139
+        t["kc"], t["vc"] = _compress_kv(a, t["qkv"], B, N, HW)
     q3 = t["qkv"].view(M, 3, H, D)
     st = (3 * C, D)
     if kept is None:
+        k, v, kst, Nk = _self_kv(t, B, H, N)
         t["ao1"], t["lse1"] = torch.empty((M, C), **bf), torch.empty((B, H, N), **f32)
-        lib.flash_attn(q3[:, 0], q3[:, 1], q3[:, 2], t["ao1"], B=B, H=H, Nq=N, Nk=N, kv_rows=M, q_strides=st, k_strides=st,
-                       v_strides=st, scale=a.scale, lse=t["lse1"], fp32_p=_fp32_p(a))
+        lib.flash_attn(q3[:, 0], k, v, t["ao1"], B=B, H=H, Nq=N, Nk=Nk, kv_rows=B * Nk, q_strides=st, k_strides=kst,
+                       v_strides=kst, scale=a.scale, lse=t["lse1"], fp32_p=_fp32_p(a))
     else:
         t["ao1"], t["lse1"] = kept["ao1"], kept["lse1"]
     t["x1"], t["y1"] = torch.empty((M, C), **f32), torch.empty((M, C), **bf)
@@ -708,39 +430,41 @@ def _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, 
 
 
 _SAVED = ("xn1", "qkv", "ao1", "lse1", "y1", "x1", "xb", "qx", "kv", "ao2", "lse2", "x2", "xn2", "h", "pre", "y3")
+_SAVED_EXTRA = ("qkv_pre", "kc", "vc")              # only blocks with qk_norm / KV compression have them
 _KEPT = ("ao1", "lse1", "ao2", "lse2")
 
 
 class BlockFn(torch.autograd.Function):
-    """One PixArtMSBlock (PixArtMS.py:71-79, no KV compression / qk_norm) as a SINGLE autograd node: the forward is the
-    kernel sequence of `_block_forward_kernels`, the backward the explicit reverse sequence of backward kernels.
+    """One PixArtMSBlock (PixArtMS.py:71-79) as a SINGLE autograd node: the forward is the kernel sequence of
+    `_block_forward_kernels`, the backward the explicit reverse sequence of backward kernels.
 
-    With one autograd node per op (the functions above) the training step carries ~100 small torch kernels per
-    block -- zero fills and slice assignments for the modulation gradients, the gradient additions where the residual
-    stream forks, bf16 casts, the accumulation of every weight gradient.
-    Here the residual-stream gradient is threaded through the backward kernels (`ln_modulate_bwd(add_in=...)`,
-    `gate_residual_fwd` as the fp32 + bf16 add), the six modulation gradients land in slices of ONE (6, B, C) buffer, and
-    the weight / bias gradients go straight into their bucket views.  Activation checkpointing is built in (`ckpt`): only
-    the block input, the conditioning and the two attention outputs + statistics are kept, the rest is recomputed here."""
+    One autograd node per op would carry ~100 small torch kernels per block -- zero fills and slice assignments for the
+    modulation gradients, the gradient additions where the residual stream forks, bf16 casts, the accumulation of every
+    weight gradient.  Here the residual-stream gradient is threaded through the backward kernels
+    (`ln_modulate_bwd(add_in=...)`, `gate_residual_fwd` as the fp32 + bf16 add), the six modulation gradients land in
+    slices of ONE (6, B, C) buffer, and the weight / bias gradients of the projections go straight into their bucket views
+    (those of q_norm / k_norm / sr / norm go through autograd).  Activation checkpointing is built in (`ckpt`): only the
+    block input, the conditioning and the two attention outputs + statistics are kept, the rest (compressed keys / values
+    included) is recomputed here."""
 
     @staticmethod
-    def forward(ctx, blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, ckpt, *params):
+    def forward(ctx, blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, HW, ckpt, *params):
         x32, cond, mod = x32.contiguous(), cond.contiguous(), mod.contiguous()
-        t = _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N)
-        names = (_KEPT if ckpt else _SAVED) + tuple(k for k in t if k.startswith("u_"))
+        t = _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, HW)
+        names = (_KEPT if ckpt else _SAVED + tuple(k for k in _SAVED_EXTRA if k in t)) + tuple(k for k in t if k.startswith("u_"))
         ctx.save_for_backward(x32, cond, mod, kv_len, kv_off, *[t[k] for k in names], *params)
-        ctx.meta = (blk, max_keys, B, N, bool(ckpt), names)
+        ctx.meta = (blk, max_keys, B, N, HW, bool(ckpt), names)
         return t["x3"]
 
     @staticmethod
     def backward(ctx, dout):
-        blk, max_keys, B, N, ckpt, names = ctx.meta
+        blk, max_keys, B, N, HW, ckpt, names = ctx.meta
         saved = ctx.saved_tensors
         x32, cond, mod, kv_len, kv_off = saved[:5]
         t = dict(zip(names, saved[5:5 + len(names)]))
         params = saved[5 + len(names):]
         if ckpt:
-            t = _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, kept=t)
+            t = _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, HW, kept=t)
         a, ca, mlp = blk.attn, blk.cross_attn, blk.mlp
         C, H = blk.hidden_size, a.num_heads
         D, M, dev = C // H, B * N, x32.device
@@ -749,7 +473,7 @@ class BlockFn(torch.autograd.Function):
         ms = mod.stride(0)
         dout = dout.contiguous()
         dm = torch.zeros((6, B, C), **f32)                # d(shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp)
-        needs = ctx.needs_input_grad[10:]
+        needs = ctx.needs_input_grad[11:]
         grads = {}
 
         def lin_bwd(tag, x, lin_mod, dy, need_dx=True, v=None):
@@ -789,28 +513,36 @@ class BlockFn(torch.autograd.Function):
         dy1 = torch.empty((M, C), **bf)
         lib.gate_residual_bwd(dx1, t["y1"], mod[:, 2], dy1, dm[2], gate_batch_stride=ms, rows_per_batch=N)
         dao1 = lin_bwd("proj", t["ao1"], a.proj, dy1)
-        dqkv = torch.empty_like(t["qkv"])
+        compressed = a.sr_ratio > 1
+        dqkv = torch.zeros_like(t["qkv"]) if compressed else torch.empty_like(t["qkv"])  # k / v rows no kept key reads: 0
         q3, g3 = t["qkv"].view(M, 3, H, D), dqkv.view(M, 3, H, D)
         st = (3 * C, D)
-        lib.flash_attn_bwd(q3[:, 0], q3[:, 1], q3[:, 2], t["ao1"], dao1, t["lse1"], g3[:, 0], g3[:, 1], g3[:, 2], B=B, H=H, Nq=N,
-                           Nk=N, kv_rows=M, q_strides=st, k_strides=st, v_strides=st, dq_strides=st, dk_strides=st, dv_strides=st,
+        k, v, kst, Nk = _self_kv(t, B, H, N)
+        dk, dv = (torch.empty_like(k), torch.empty_like(v)) if compressed else (g3[:, 1], g3[:, 2])
+        lib.flash_attn_bwd(q3[:, 0], k, v, t["ao1"], dao1, t["lse1"], g3[:, 0], dk, dv, B=B, H=H, Nq=N, Nk=Nk, kv_rows=B * Nk,
+                           q_strides=st, k_strides=kst, v_strides=kst, dq_strides=st, dk_strides=kst, dv_strides=kst,
                            scale=a.scale)
+        kv_grads = _compress_kv_bwd(a, t["qkv"], dk, dv, dqkv, B, N, HW) if compressed else []
+        qk_grads = []
+        if _norms_qk(a):
+            # LN-modulate backward with one "sample" spanning all rows and scale = weight - 1: its dscale / dshift column sums
+            # are the gradients of weight / bias
+            for i, (ln, w) in enumerate(((a.q_norm, params[28]), (a.k_norm, params[30]))):
+                xs = t["qkv_pre"][:, i * C:(i + 1) * C].float().contiguous()
+                dxs = torch.empty_like(xs)
+                dsh, dsc = torch.zeros((1, C), **f32), torch.zeros((1, C), **f32)
+                lib.ln_modulate_bwd(xs, dqkv[:, i * C:(i + 1) * C].contiguous(), (w.float() - 1.0).view(1, C).contiguous(), dxs,
+                                    dsh, dsc, mod_batch_stride=C, rows_per_batch=M, eps=ln.eps)
+                dqkv[:, i * C:(i + 1) * C] = dxs
+                qk_grads += [dsc.view(C), dsh.view(C)]
         dxn1 = lin_bwd("qkv", t["xn1"], a.qkv, dqkv)
         dx = torch.empty((M, C), **f32)
         lib.ln_modulate_bwd(x32, dxn1, mod[:, 1], dx, dm[0], dm[1], mod_batch_stride=ms, rows_per_batch=N, add_in=dx1)
         pg = [g for tag in _TAGS for g in grads[tag]]
-        return (None, dx, dcond, dm.permute(1, 0, 2), None, None, None, None, None, None, *pg)
+        pg += [g.to(p.dtype) if n else None for g, p, n in zip(qk_grads + kv_grads, params[28:], needs[28:])]
+        return (None, dx, dcond, dm.permute(1, 0, 2), None, None, None, None, None, None, None, *pg)
 
 
 def block_train(blk, x32, cond, kv_len, kv_off, max_keys, mod, B, N, HW, ckpt: bool):
-    """Training forward of one block: the single-node form where it applies, else the per-op functions (with torch's
-    activation checkpointing around them when `ckpt`)."""
-    plain = blk.attn.sr_ratio == 1 and isinstance(blk.attn.q_norm, torch.nn.Identity)
-    if _BLOCK_FN and plain:
-        _, params = _block_params(blk)
-        return BlockFn.apply(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, ckpt, *params)
-    if ckpt:
-        from torch.utils.checkpoint import checkpoint
-        return checkpoint(block_forward_train, blk, x32, cond, kv_len, kv_off, max_keys, mod, B, N, {}, HW, use_reentrant=False,
-                          preserve_rng_state=False)
-    return block_forward_train(blk, x32, cond, kv_len, kv_off, max_keys, mod, B, N, None, HW)
+    """Training forward of one block: one BlockFn node, activation-checkpointed when `ckpt`."""
+    return BlockFn.apply(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, tuple(HW), ckpt, *_block_params(blk))

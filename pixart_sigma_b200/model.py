@@ -723,12 +723,11 @@ class PixArtMS(nn.Module):
         return self.unpatchify(out).to(self.output_dtype or dt)
 
     def _forward_train(self, x, timestep, y, mask=None, data_info=None):
-        """The same forward recorded for autograd (train_scripts/train.py:189-197): every block op is a
+        """The same forward recorded for autograd (train_scripts/train.py:189-197): every block is one
         `torch.autograd.Function` over the sm_90a kernels (autograd.py), blocks marked by `set_grad_checkpoint`
         (diffusion/model/utils.py:28-45) are activation-checkpointed like PixArtMS.py:206.  Parameters may be fp32
         (mixed precision: the kernels read cached bf16 shadows) or bf16.  Unmerged LoRA adapters are applied: on the kernel
         path through the GEMM K-tail (operands rebuilt here from the parameters), on the fp32 torch glue in fp32."""
-        from torch.utils.checkpoint import checkpoint
         from . import autograd as ag
         w0 = self.blocks[0].attn.qkv.weight
         if not w0.is_cuda:
@@ -772,7 +771,7 @@ class PixArtMS(nn.Module):
             mod = blk.scale_shift_table.float()[None] + t0
             if self.training and blk.drop_path_rate > 0:        # drawn here, outside the (recomputed) checkpointed function
                 mod = _drop_path_gates(mod, blk.drop_path_rate)
-            # one autograd node per block (autograd.BlockFn, activation checkpointing built in) where it applies
+            # one autograd node per block (autograd.BlockFn, activation checkpointing built in)
             x32 = ag.block_train(blk, x32, cond, kv_len, None, L, mod, B, N, (self.h, self.w),
                                  bool(getattr(blk, "grad_checkpointing", False)))
 

@@ -38,6 +38,9 @@ def _rounded(sd):
 def _build_train(cfg, sd, dtype=torch.float32, checkpoint=False):
     kw = dict(type="PixArtMS", depth=cfg.depth, hidden_size=cfg.hidden_size, num_heads=cfg.num_heads,
               input_size=cfg.input_size, pe_interpolation=cfg.pe_interpolation, model_max_length=cfg.model_max_length)
+    if cfg.kv_sampling is not None:
+        kw["kv_compress_config"] = dict(sampling=cfg.kv_sampling, scale_factor=cfg.kv_scale_factor,
+                                        kv_compress_layer=list(cfg.kv_compress_layer))
     with torch.device("cuda"):
         m = build_model(kw, use_grad_checkpoint=checkpoint)
     m.load_state_dict(sd, strict=False)
@@ -79,10 +82,28 @@ def test_block_gradients_match_oracle(B, hw, lens):
     assert max(errs.values()) < 2e-2, errs
 
 
-@pytest.mark.parametrize("sampling", ["conv", "uniform"])
+def _kernel_block_grads(blk, x, ycat, t0, dout, lens, hw, ckpt):
+    """(output, {"x": x.grad, parameter name: .grad}) of one kernel block forward + backward, activation-checkpointed or not."""
+    blk.grad_checkpointing = ckpt
+    blk.zero_grad(set_to_none=True)
+    xk = x.clone().cuda().requires_grad_(True)
+    got = blk(xk, ycat.cuda()[None], t0.cuda(), lens, hw)
+    got.backward(dout.cuda())
+    return got.detach().cpu(), {"x": xk.grad.cpu(), **{n: p.grad.float().cpu() for n, p in blk.named_parameters()}}
+
+
+def _assert_checkpointing_agrees(blk, x, ycat, t0, dout, lens, hw, grads):
+    """The checkpointed block gives the gradients `grads` of the plain one (atomics reorder sums)."""
+    _, ck = _kernel_block_grads(blk, x, ycat, t0, dout, lens, hw, True)
+    for n in grads:
+        assert torch.equal(ck[n], grads[n]) or po.rel_err(ck[n], grads[n]) < 1e-5, (n, po.rel_err(ck[n], grads[n]))
+
+
+@pytest.mark.parametrize("sampling", ["conv", "uniform", "uniform_every"])
 def test_kv_compressed_block_gradients_match_oracle(sampling):
     """Training through a KV-compressed block (PixArt_blocks.py:97-121, 137-139): conv + LN compression kernel and its
-    backward, attention backward with Nk = N / 4."""
+    backward, attention backward with Nk = N / 4 (N / 2 for uniform_every); then the activation-checkpointed block against
+    the plain one."""
     B, hw, lens, C = 2, (16, 16), [300, 9], 1152
     N = hw[0] * hw[1]
     cfg = po.OracleConfig(depth=1, kv_sampling=sampling, kv_scale_factor=2, kv_compress_layer=[0])
@@ -102,21 +123,21 @@ def test_kv_compressed_block_gradients_match_oracle(sampling):
     xo = x.clone().requires_grad_(True)
     want = po.block_forward(sdo, "blocks.0", xo, ycat[None], t0, lens, hw, 16, 2, sampling)
     want.backward(dout)
-    xk = x.clone().cuda().requires_grad_(True)
-    got = blk(xk, ycat.cuda()[None], t0.cuda(), lens, hw)
-    ferr = po.rel_err(got.detach().cpu(), want.detach())
+    got, grads = _kernel_block_grads(blk, x, ycat, t0, dout, lens, hw, False)
+    ferr = po.rel_err(got, want.detach())
     assert ferr < 2e-3, ferr
-    got.backward(dout.cuda())
-    errs = {"x": po.rel_err(xk.grad.cpu(), xo.grad)}
-    for n, p in blk.named_parameters():
-        errs[n] = po.rel_err(p.grad.float().cpu(), sdo["blocks.0." + n].grad)
+    errs = {"x": po.rel_err(grads["x"], xo.grad)}
+    for n, _ in blk.named_parameters():
+        errs[n] = po.rel_err(grads[n], sdo["blocks.0." + n].grad)
     _log(f"kv-compressed ({sampling}) block grads: fwd={ferr:.2e} " + " ".join(f"{k}={v:.2e}" for k, v in errs.items()))
     assert max(errs.values()) < 2e-2, errs
+    _assert_checkpointing_agrees(blk, x, ycat, t0, dout, lens, hw, grads)
 
 
 def test_qk_norm_block_gradients_match_oracle():
     """Training with qk_norm=True (PixArt_blocks.py:133-134): q_norm / k_norm on the qkv GEMM output, their backward through the
-    LayerNorm-modulate backward kernel (autograd.QkNormFn)."""
+    LayerNorm-modulate backward kernel, inside autograd.BlockFn; then the activation-checkpointed block against the plain
+    one."""
     B, hw, lens, C = 2, (16, 16), [300, 40], 1152
     N = hw[0] * hw[1]
     cfg = po.OracleConfig(depth=1, qk_norm=True)
@@ -135,21 +156,20 @@ def test_qk_norm_block_gradients_match_oracle():
     xo = x.clone().requires_grad_(True)
     want = po.block_forward(sdo, "blocks.0", xo, ycat[None], t0, lens, hw, 16, 1, None, True)
     want.backward(dout)
-    xk = x.clone().cuda().requires_grad_(True)
-    got = blk(xk, ycat.cuda()[None], t0.cuda(), lens, hw)
-    ferr = po.rel_err(got.detach().cpu(), want.detach())
+    got, grads = _kernel_block_grads(blk, x, ycat, t0, dout, lens, hw, False)
+    ferr = po.rel_err(got, want.detach())
     assert ferr < 2e-3, ferr
-    got.backward(dout.cuda())
-    errs = {"x": po.rel_err(xk.grad.cpu(), xo.grad)}
-    for n, p in blk.named_parameters():
+    errs = {"x": po.rel_err(grads["x"], xo.grad)}
+    for n, _ in blk.named_parameters():
         if n == "attn.k_norm.bias":
             # a constant added to every key moves all logits of a query by the same amount: the exact gradient is ZERO and both
             # sides hold rounding noise only -- compare its size with the (real) gradient of q_norm.bias instead
-            errs[n] = (p.grad.float().norm() / blk.attn.q_norm.bias.grad.float().norm()).item()
+            errs[n] = (grads[n].norm() / grads["attn.q_norm.bias"].norm()).item()
             continue
-        errs[n] = po.rel_err(p.grad.float().cpu(), sdo["blocks.0." + n].grad)
+        errs[n] = po.rel_err(grads[n], sdo["blocks.0." + n].grad)
     _log(f"qk_norm block grads: fwd={ferr:.2e} " + " ".join(f"{k}={v:.2e}" for k, v in errs.items()))
     assert max(errs.values()) < 2e-2, errs
+    _assert_checkpointing_agrees(blk, x, ycat, t0, dout, lens, hw, grads)
 
 
 def _oracle_step(cfg, sd, x0, t, y, mask, noise):
@@ -160,7 +180,7 @@ def _oracle_step(cfg, sd, x0, t, y, mask, noise):
     return {k: v.detach() for k, v in terms.items()}, {k: v.grad for k, v in sdo.items() if v.grad is not None}
 
 
-@pytest.mark.parametrize("name", ["train_d2_b2", "train_d2_b3_512"])
+@pytest.mark.parametrize("name", ["train_d2_b2", "train_d2_b3_512", "train_d2_kvconv"])
 def test_train_step_matches_oracle_and_reference_fixture(golden_dir, name):
     fix = torch.load(os.path.join(golden_dir, name + ".pt"))
     cfg = po.OracleConfig(**fix["cfg"])
