@@ -136,8 +136,14 @@ def kv_downsample(sd, prefix: str, t: Tensor, H: int, W: int, sr: int, sampling:
     if sampling is None or sr == 1:
         return t
     B, N, C = t.shape
+    # the reference reshapes the [::sr] picks to int(N / sr) (int(H / sr) x int(W / sr)) tokens, which fails unless sr
+    # divides the grid (:103, :107-108, :121)
     if sampling == "uniform_every":
+        if N % sr:
+            raise ValueError(f"'uniform_every' KV sampling needs the token count {N} to be a multiple of scale_factor {sr}")
         return t[:, ::sr]
+    if sampling == "uniform" and (H % sr or W % sr):
+        raise ValueError(f"'uniform' KV sampling needs scale_factor {sr} to divide the token grid {H} x {W}")
     img = t.reshape(B, H, W, C).permute(0, 3, 1, 2)
     if sampling == "ave":      # NB: the reference calls nearest-neighbour interpolation "ave" (:109-112)
         out = F.interpolate(img, scale_factor=1 / sr, mode="nearest").permute(0, 2, 3, 1)

@@ -35,6 +35,7 @@ from typing import Optional
 import torch
 
 from . import lib
+from .model import check_kv_conv_grid, kv_pick
 
 
 def _shadow(mod: torch.nn.Module, kind: str) -> Optional[torch.Tensor]:
@@ -313,26 +314,15 @@ def _block_params(blk):
     return tuple(t for m in mods for t in (m.weight, m.bias, *_lora_params(m))) + tuple(t for m in extra for t in (m.weight, m.bias))
 
 
-def _kv_pick(a, x, B, N, HW):
-    """The rows of x (B*N, C) that a parameter-free KV compression keeps (PixArt_blocks.py:97-121), as a strided view."""
-    sr = a.sr_ratio
-    if a.sampling == "uniform_every":
-        return x.view(B, N, -1)[:, ::sr]
-    if a.sampling in ("uniform", "ave"):           # the reference's 'ave' is nearest-neighbour = the same strided pick
-        return x.view(B, HW[0], HW[1], -1)[:, ::sr, ::sr]
-    raise ValueError(a.sampling)
-
-
 def _compress_kv(a, qkv, B, N, HW):
     """(kc, vc) (B*Nk, C): the compressed keys / values of the qkv GEMM output.  'conv' (scale factor 2) runs the fused
-    conv + LN kernel; the parameter-free samplings are strided picks (pure data movement, torch)."""
+    conv + LN kernel; the parameter-free samplings are strided picks (`model.kv_pick`, pure data movement, torch)."""
     C3 = qkv.shape[1]
     C = C3 // 3
     k, v = qkv[:, C:2 * C], qkv[:, 2 * C:]
     if a.sampling != "conv":
-        return tuple(_kv_pick(a, x, B, N, HW).contiguous().view(-1, C) for x in (k, v))
-    if a.sr_ratio != 2:
-        raise NotImplementedError("conv KV compression kernel is specialised for scale_factor 2")
+        return tuple(kv_pick(x, B, HW, a.sampling, a.sr_ratio).contiguous().view(-1, C) for x in (k, v))
+    check_kv_conv_grid(HW, a.sr_ratio)
     Hh, Ww = HW
     n_out = (Hh // 2) * (Ww // 2)
     kc = torch.empty((B * n_out, C), dtype=torch.bfloat16, device=qkv.device)
@@ -349,7 +339,7 @@ def _compress_kv_bwd(a, qkv, dkc, dvc, dqkv, B, N, HW):
     C = C3 // 3
     if a.sampling != "conv":
         for d, dx in ((dkc, dqkv[:, C:2 * C]), (dvc, dqkv[:, 2 * C:])):
-            pick = _kv_pick(a, dx, B, N, HW)
+            pick = kv_pick(dx, B, HW, a.sampling, a.sr_ratio)
             pick.copy_(d.view(pick.shape))
         return []
     g = [torch.zeros(p.shape, dtype=torch.float32, device=qkv.device) for p in (a.sr.weight, a.sr.bias, a.norm.weight, a.norm.bias)]

@@ -203,6 +203,41 @@ class AttentionKVCompress(nn.Module):
             self.q_norm, self.k_norm = nn.Identity(), nn.Identity()
 
 
+def kv_pick(t: torch.Tensor, B: int, HW: Tuple[int, int], sampling: str, sr: int) -> torch.Tensor:
+    """The keys / values a parameter-free KV compression keeps (downsample_2d, PixArt_blocks.py:97-121), as a strided view
+    of t (B*H*W, C): (B, H', W', C) for 'uniform' / 'ave', (B, N', C) for 'uniform_every'.  The inference forward copies it
+    out, the training backward scatters into it.
+
+    'ave' is nearest-neighbour interpolation by 1/sr (:109-112): rows and columns 0, sr, .., sr (floor(H/sr) - 1), a
+    floor(H/sr) x floor(W/sr) grid.  'uniform' / 'uniform_every' are the [::sr] pick, which the reference then reshapes to
+    floor(H/sr) x floor(W/sr) (floor(N/sr)) tokens: it fails unless sr divides the grid, and so does this, with a ValueError
+    instead of silently keeping ceil(H/sr) x ceil(W/sr) keys."""
+    Hh, Ww = HW
+    C = t.shape[-1]
+    if sampling == "uniform_every":
+        if (Hh * Ww) % sr:
+            raise ValueError(f"'uniform_every' KV sampling needs the token count {Hh * Ww} to be a multiple of scale_factor {sr}")
+        return t.view(B, Hh * Ww, C)[:, ::sr]
+    if sampling == "uniform":
+        if Hh % sr or Ww % sr:
+            raise ValueError(f"'uniform' KV sampling needs scale_factor {sr} to divide the token grid {Hh} x {Ww}")
+        return t.view(B, Hh, Ww, C)[:, ::sr, ::sr]
+    if sampling == "ave":
+        Ho, Wo = Hh // sr, Ww // sr
+        if Ho == 0 or Wo == 0:
+            raise ValueError(f"'ave' KV sampling by scale_factor {sr} leaves no keys on a {Hh} x {Ww} token grid")
+        return t.view(B, Hh, Ww, C)[:, :Ho * sr:sr, :Wo * sr:sr]
+    raise ValueError(f"unknown KV sampling {sampling!r}")
+
+
+def check_kv_conv_grid(HW: Tuple[int, int], sr: int) -> None:
+    """The fused conv + LayerNorm KV compression kernel takes scale_factor 2 on an even token grid only."""
+    if sr != 2:
+        raise NotImplementedError("conv KV compression kernel is specialised for scale_factor 2")
+    if HW[0] % 2 or HW[1] % 2:
+        raise NotImplementedError(f"conv KV compression kernel needs an even token grid (got {HW[0]} x {HW[1]})")
+
+
 # ------------------------------------------------------------------------------------------------- workspace
 class _Workspace:
     """Activation buffers reused by all 28 blocks of one forward (owned by the model, sized on first use)."""
@@ -495,21 +530,14 @@ class PixArtMSBlock(nn.Module):
         sr, dev = a.sr_ratio, qkv.device
         k_in, v_in = qkv[:, C:2 * C], qkv[:, 2 * C:]
         if a.sampling == "conv":
-            if sr != 2:
-                raise NotImplementedError("conv KV compression kernel is specialised for scale_factor 2")
+            check_kv_conv_grid(HW, sr)
             n_out = (Hh // 2) * (Ww // 2)
             kc = ws.get("k_comp", (B, n_out, C), torch.bfloat16, dev)
             vc = ws.get("v_comp", (B, n_out, C), torch.bfloat16, dev)
             lib.kv_compress(k_in, v_in, kc, vc, a.sr.weight, a.sr.bias, a.norm.weight, a.norm.bias, B=B, H=Hh, W=Ww,
                             ld_in=qkv.stride(0), eps=a.norm.eps)
             return kc.view(-1, C), vc.view(-1, C), n_out
-        if a.sampling == "uniform_every":
-            pick = lambda t: t.reshape(B, N, C)[:, ::sr].contiguous()
-        elif a.sampling in ("uniform", "ave"):     # the reference's 'ave' is nearest-neighbour = the same strided pick
-            pick = lambda t: t.reshape(B, Hh, Ww, C)[:, ::sr, ::sr].contiguous()
-        else:
-            raise ValueError(a.sampling)
-        kc, vc = pick(k_in), pick(v_in)
+        kc, vc = (kv_pick(t, B, HW, a.sampling, sr).contiguous() for t in (k_in, v_in))
         n_out = kc.numel() // (B * C)
         return kc.view(-1, C), vc.view(-1, C), n_out
 

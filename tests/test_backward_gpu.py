@@ -185,8 +185,7 @@ def _attn_ref(q, k, v, lens, scale):
     (1, 2, 128, 128, None), (2, 3, 256, 256, None), (1, 16, 1024, 1024, None), (2, 2, 256, 64, None),
     (2, 2, 128, 300, [300, 77]), (3, 4, 256, 300, [5, 130, 256]), (2, 2, 200, 200, None), (1, 3, 4032, 4032, None),
     (2, 2, 72, 300, [300, 41]), (2, 2, 201, 130, None), (1, 3, 1089, 1089, None),     # Nq % 4 != 0: no TMA copies of lse / delta
-    # more work items than SMs (a persistent launch, PXA_BWD_PERSISTENT=1, then walks 2 items per CTA with the barrier phases and
-    # the ring position carried over), ragged packed keys with skipped key tiles in between
+    # more (128-row tile, head, sample) CTAs than SMs, ragged key lengths whose samples end inside a key tile
     (2, 16, 1024, 1024, None), (4, 16, 640, 300, [300, 77, 65, 130]), (3, 16, 516, 516, None),
 ])
 def test_flash_attn_backward(B, H, Nq, Nk, lens):
