@@ -166,8 +166,9 @@ def test_every_binding_checks_its_return_code_with_one_label():
 
 def test_hi_lo_split_of_p_carries_sixteen_mantissa_bits():
     """The arithmetic behind `PxaAttnArgs.p_precision = 1` (KERNELS.md): P_hi = bf16(P), P_lo = bf16(P - P_hi) -- the difference is
-    exact in fp32 -- so P_hi + P_lo reproduces P to 2^-17 relative (one bf16 term: up to 2^-8), for P anywhere in the lazy-rescale range
-    (0, 2^8] incl. values whose low term is subnormal-small."""
+    exact in fp32 -- so P_hi + P_lo reproduces P to 2^-17 relative (one bf16 term: up to 2^-8), for P in (0, 2^8] -- wider than
+    the (0, 1] the forward produces, since it rescales by the running max every block -- incl. values whose low term is
+    subnormal-small."""
     g = torch.Generator().manual_seed(0)
     p = torch.exp2(torch.rand(1 << 16, generator=g) * 40 - 32)                 # 2^-32 .. 2^8
     hi = p.to(torch.bfloat16)

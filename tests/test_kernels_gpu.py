@@ -329,7 +329,8 @@ def test_flash_attn_interleaved_qkv_buffer(variant):
 
 @pytest.mark.parametrize("variant", [2, 3, 4])
 def test_flash_attn_large_logits_trigger_rescale(variant):
-    """Keys ordered so the running max keeps growing by > 2^8 between blocks: exercises the lazy O rescale."""
+    """Keys ordered so the running max keeps growing from block to block: every block's O / l rescale by corr changes the
+    result."""
     B, H, N = 1, 2, 512
     q = _randn(B, N, H, 72, seed=34)
     k = _randn(B, N, H, 72, seed=35)

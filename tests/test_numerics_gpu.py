@@ -363,8 +363,8 @@ def _one_key_problem(lens, Nq, H, D, seed, alpha):
 @pytest.mark.parametrize("fp32_p", [False, True])
 def test_flash_attn_one_key_per_query_exact(layout, fp32_p):
     """q_i = 8 k_pi(i) with +-1 keys: the chosen logit beats every other valid key by more than 8 in log2 units (asserted),
-    so when its key block arrives the running max moves by more than the lazy-rescale threshold, the max becomes that logit
-    and its P is exp2(0) = 1 exactly; every other P is < 2^-margin.  The normaliser is then 1 + (< 2^-20), and with
+    so when its key block arrives the running max becomes that logit (the forward takes the max and rescales O by corr in
+    every block) and its P is exp2(0) = 1 exactly; every other P is < 2^-margin.  The normaliser is then 1 + (< 2^-20), and with
     1/2 <= |v| < 3/2 the other keys add < 2^-30 |v[pi(i)]|, far below half a bf16 ulp, so out[i] == v[pi(i)] bit for bit (a v
     element of 0 would instead receive those tiny terms, correctly, and is therefore excluded), and lse[i] = logit * log2 e to fp32 accuracy.  pi maps onto every valid
     key (keys 63 / 64 / 127 / 128 and the partial last block included); ragged kv_len with an empty sample (zero output), 16
