@@ -259,8 +259,9 @@ typedef struct PxaAdamWArgs {
   void* shadow_bf16;     /* bf16 [n] or NULL                    */
   int64_t n;             /* multiple of 4                       */
   int32_t step;          /* 1-based step count (bias correction) */
-  float lr, beta1, beta2, eps, weight_decay;
   float grad_scale;      /* gradients are multiplied by this first (1 / loss scale, or 1) */
+  double lr, beta1, beta2, eps, weight_decay;   /* as torch.optim.AdamW takes them: 1 - beta and the bias corrections
+                                                   are formed in double, then rounded once to fp32 */
 } PxaAdamWArgs;
 int pxa_adamw_flat(const PxaAdamWArgs* args, void* stream);
 

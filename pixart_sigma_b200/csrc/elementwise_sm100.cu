@@ -733,8 +733,8 @@ namespace pxa {
 // (+ 2 B) written per parameter.
 __global__ void __launch_bounds__(256) adamw_flat_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                          float* __restrict__ v, __nv_bfloat16* __restrict__ shadow, long long n4,
-                                                         float lr, float beta1, float beta2, float eps, float decay,
-                                                         float step_size, float inv_sqrt_bc2, float grad_scale) {
+                                                         float beta1, float omb1, float beta2, float omb2, float eps,
+                                                         float decay, float step_size, float inv_sqrt_bc2, float grad_scale) {
   for (long long i = blockIdx.x * 256LL + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
     float4 pv = reinterpret_cast<float4*>(p)[i];
     const float4 gv = reinterpret_cast<const float4*>(g)[i];
@@ -744,8 +744,8 @@ __global__ void __launch_bounds__(256) adamw_flat_kernel(float* __restrict__ p, 
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const float gk = gp[k] * grad_scale;
-      mp[k] = fmaf(beta1, mp[k], (1.0f - beta1) * gk);
-      vp[k] = fmaf(beta2, vp[k], (1.0f - beta2) * gk * gk);
+      mp[k] = fmaf(beta1, mp[k], omb1 * gk);
+      vp[k] = fmaf(beta2, vp[k], omb2 * gk * gk);
       const float denom = sqrtf(vp[k]) * inv_sqrt_bc2 + eps;
       pp[k] = fmaf(-step_size, mp[k] / denom, pp[k] * decay);
     }
@@ -770,14 +770,17 @@ extern "C" int pxa_adamw_flat(const PxaAdamWArgs* args, void* stream) {
        reinterpret_cast<uintptr_t>(a.exp_avg_sq)) & 15 || (reinterpret_cast<uintptr_t>(a.shadow_bf16) & 7))
     return fail(PXA_ERR_ALIGN, "param / grad / exp_avg / exp_avg_sq must be 16-byte aligned, shadow_bf16 8-byte");
   PXA_REQUIRE_SM90();
-  const double bc1 = 1.0 - pow((double)a.beta1, (double)a.step), bc2 = 1.0 - pow((double)a.beta2, (double)a.step);
+  // 1 - beta, the bias corrections and the decay factor from the double hyper-parameters, as torch.optim.AdamW forms them:
+  // 1.0f - 0.999f is 0.99998713e-3, 1.3e-5 away from 1e-3, and so is a bias correction taken from the fp32 beta2
+  const double bc1 = 1.0 - pow(a.beta1, (double)a.step), bc2 = 1.0 - pow(a.beta2, (double)a.step);
   const long long n4 = a.n / 4;
   long long blocks = (n4 + 255) / 256;
   const long long cap = 16LL * device_info().sms;
   if (blocks > cap) blocks = cap;
   adamw_flat_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      a.param, a.grad, a.exp_avg, a.exp_avg_sq, reinterpret_cast<__nv_bfloat16*>(a.shadow_bf16), n4, a.lr, a.beta1, a.beta2, a.eps,
-      1.0f - a.lr * a.weight_decay, (float)(a.lr / bc1), (float)(1.0 / sqrt(bc2)), a.grad_scale);
+      a.param, a.grad, a.exp_avg, a.exp_avg_sq, reinterpret_cast<__nv_bfloat16*>(a.shadow_bf16), n4, (float)a.beta1,
+      (float)(1.0 - a.beta1), (float)a.beta2, (float)(1.0 - a.beta2), (float)a.eps, (float)(1.0 - a.lr * a.weight_decay),
+      (float)(a.lr / bc1), (float)(1.0 / sqrt(bc2)), a.grad_scale);
   launch_counter()++;
   PXA_CHECK_CUDA(cudaGetLastError());
   return PXA_OK;

@@ -61,8 +61,8 @@ class MlpArgs(C.Structure):
 
 class AdamWArgs(C.Structure):
     _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
-                ("shadow_bf16", C.c_void_p), ("n", C.c_int64), ("step", C.c_int32), ("lr", C.c_float), ("beta1", C.c_float),
-                ("beta2", C.c_float), ("eps", C.c_float), ("weight_decay", C.c_float), ("grad_scale", C.c_float)]
+                ("shadow_bf16", C.c_void_p), ("n", C.c_int64), ("step", C.c_int32), ("grad_scale", C.c_float), ("lr", C.c_double),
+                ("beta1", C.c_double), ("beta2", C.c_double), ("eps", C.c_double), ("weight_decay", C.c_double)]
 
 
 GRAD_CLIP_PARTS, GRAD_CLIP_MAX_BUCKETS = 1024, 128
