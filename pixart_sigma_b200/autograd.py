@@ -516,13 +516,15 @@ class BlockFn(torch.autograd.Function):
         qk_grads = []
         if _norms_qk(a):
             # LN-modulate backward with one "sample" spanning all rows and scale = weight - 1: its dscale / dshift column sums
-            # are the gradients of weight / bias
-            for i, (ln, w) in enumerate(((a.q_norm, params[28]), (a.k_norm, params[30]))):
+            # are the gradients of weight / bias.  The weight is the bf16 shadow the forward's layernorm_affine_ used, not an
+            # fp32 master weight: dx is the derivative of the function the forward computed (w - 1 is exact in fp32).
+            for i, ln in enumerate((a.q_norm, a.k_norm)):
                 xs = t["qkv_pre"][:, i * C:(i + 1) * C].float().contiguous()
                 dxs = torch.empty_like(xs)
                 dsh, dsc = torch.zeros((1, C), **f32), torch.zeros((1, C), **f32)
-                lib.ln_modulate_bwd(xs, dqkv[:, i * C:(i + 1) * C].contiguous(), (w.float() - 1.0).view(1, C).contiguous(), dxs,
-                                    dsh, dsc, mod_batch_stride=C, rows_per_batch=M, eps=ln.eps)
+                scale = (_shadow(ln, "w").float() - 1.0).view(1, C)
+                lib.ln_modulate_bwd(xs, dqkv[:, i * C:(i + 1) * C].contiguous(), scale, dxs, dsh, dsc, mod_batch_stride=C,
+                                    rows_per_batch=M, eps=ln.eps)
                 dqkv[:, i * C:(i + 1) * C] = dxs
                 qk_grads += [dsc.view(C), dsh.view(C)]
         dxn1 = lin_bwd("qkv", t["xn1"], a.qkv, dqkv)

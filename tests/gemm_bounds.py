@@ -130,6 +130,20 @@ def assert_guard(buf, M, N, name):
     assert bad == 0, f"{name}: {bad} guard elements overwritten"
 
 
+def auto_splits(M, N, K, sms):
+    """The split count launch_wgrad picks for k_splits = 0 (gemm_sm100.cu) on `sms` SMs: the most even wave."""
+    tiles = -(-M // 128) * -(-N // 128)
+    nkb = -(-K // 64)
+    best, best_eff, ks = 1, 0.0, 1
+    while ks <= 16 and nkb // ks >= 8:
+        t = tiles * ks
+        eff = t / (-(-t // sms) * sms)
+        if eff > best_eff + 1e-9:
+            best_eff, best = eff, ks
+        ks += 1
+    return min(best, nkb)
+
+
 def mn_splits(nkb, k_splits):
     """The K-block ranges [lo, hi) of the k_splits splits of nkb K-blocks, as gemm_bf16_kernel divides them."""
     return [(ks * nkb // k_splits, (ks + 1) * nkb // k_splits) for ks in range(k_splits)]

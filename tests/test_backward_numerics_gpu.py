@@ -22,6 +22,8 @@ import torch.nn.functional as F
 from test_numerics_gpu import LOG2E, SENTINEL, _assert_pad_unchanged, _ints, _ln_slack, _offset_input, _one_key_problem, _padded, \
     _randn, assert_bf16_close, bf16_ulp
 
+from norm_bounds import ln_bwd_slack as _ln_bwd_slack, ln_stats as _ln_stats, sample_sum_slack as _sample_sum_slack
+
 pytestmark = pytest.mark.gpu
 
 if torch.cuda.is_available():
@@ -64,28 +66,6 @@ def _front(rows, cols, fill, dtype, extra=3):
     """A contiguous (rows, cols) view at the front of a (rows + extra, cols) buffer filled with `fill`."""
     buf = torch.full((rows + extra, cols), fill, dtype=dtype, device=DEV)
     return buf[:rows], buf
-
-
-def _ln_bwd_slack(xh, rstd, g, r, rstd_rel):
-    """Element-wise bound on the fp32 error of dx = rstd (g - mean_c g - xh mean_c(g xh)) over the last dim, from float64
-    xh, rstd, g = dxn (1 + scale) (or dy gamma) and r = |mean| / std of the row:
-      - the kernel's xh carries e = 2^-18 (1 + r) (the row mean: a sum of C terms in <= 41 sequential fp32 additions, 36
-        per lane then 5 butterfly levels, see _ln_slack) + 2^-19 |xh| (rstd and the rounding of (x - mean) rstd); a
-        perturbation e of xh moves dx by rstd (e |mean(g xh)| + |xh| mean(|g| e));
-      - 3 rstd_rel T for the relative error of rstd, which enters dx, xh and mean(g xh) once each, and 2^-18 T for the
-        roundings of g, of the two means (<= 41 additions each) and of the final expression, where
-        T = rstd (|g| + mean|g| + |xh| mean|g xh|) bounds every term's magnitude."""
-    mg, mgx = g.mean(-1, keepdim=True), (g * xh).mean(-1, keepdim=True)
-    e = 2.0 ** -18 * (1 + r) + 2.0 ** -19 * xh.abs()
-    T = rstd * (g.abs() + g.abs().mean(-1, keepdim=True) + xh.abs() * (g * xh).abs().mean(-1, keepdim=True))
-    return (3 * rstd_rel + 2.0 ** -18) * T + rstd * (e * mgx.abs() + xh.abs() * (g.abs() * e).mean(-1, keepdim=True))
-
-
-def _ln_stats(xd, eps):
-    mean = xd.mean(-1, keepdim=True)
-    var = xd.var(-1, unbiased=False, keepdim=True)
-    rstd = 1 / torch.sqrt(var + eps)
-    return (xd - mean) * rstd, rstd, mean.abs() / var.sqrt().clamp(min=1e-30)
 
 
 # ------------------------------------------------------------------------------------------------- gate + residual
@@ -218,15 +198,6 @@ def _ln_bwd_reference(x, dxn, scale_rows, eps):
     g = dxn.double() * (1 + scale_rows)
     dx = rstd * (g - g.mean(-1, keepdim=True) - xh * (g * xh).mean(-1, keepdim=True))
     return xh, rstd, r, g, dx
-
-
-def _sample_sum_slack(b_of, B, rpb, M, terms, pre):
-    """Bound on the fp32 error of pre[b] + sum_{rows of b} terms: sequential runs of <= 16 rows per warp (<= 15 u sum|terms|),
-    then one atomic per warp that touches sample b onto pre (W_b atomics: <= W_b u (|pre| + sum|terms|))."""
-    first = torch.arange(B, device=DEV) * rpb
-    last = torch.clamp(first + rpb, max=M) - 1
-    wb = (last // 16 - first // 16 + 1).double()[:, None]
-    return (15 + wb) * U * (pre.double().abs() + torch.zeros_like(pre, dtype=torch.float64).index_add(0, b_of, terms.abs()))
 
 
 @pytest.mark.parametrize("eps", [1e-6, 1e-5])

@@ -244,19 +244,10 @@ def test_lora_tail_fused_qkv_block_diagonal():
 # ------------------------------------------------------------------------------------------------- weight gradient
 def auto_splits(M, N, K, max_ctas=0):
     """The split count launch_wgrad picks for k_splits = 0 (gemm_sm100.cu): the most even wave over the SMs."""
-    tiles = -(-M // 128) * -(-N // 128)
-    nkb = -(-K // 64)
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     if 0 < max_ctas < sms:
         sms = max_ctas
-    best, best_eff, ks = 1, 0.0, 1
-    while ks <= 16 and nkb // ks >= 8:
-        t = tiles * ks
-        eff = t / (-(-t // sms) * sms)
-        if eff > best_eff + 1e-9:
-            best_eff, best = eff, ks
-        ks += 1
-    return min(best, nkb)
+    return gb.auto_splits(M, N, K, sms)
 
 
 def check_wgrad(a_t, w_t, k_splits, name):

@@ -20,6 +20,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from norm_bounds import ln_slack as _ln_slack
+
 pytestmark = pytest.mark.gpu
 
 if torch.cuda.is_available():
@@ -552,13 +554,6 @@ def test_groupnorm_large_offsets_elementwise(B, H, W, Cc, silu, ratio):
     del xd, xhat
     assert_bf16_close(out, want, slack, name=f"groupnorm{'+silu' if silu else ''} {B}x{H}x{W}x{Cc} mean/std={ratio}",
                       max_ulp=2.0)
-
-
-def _ln_slack(xd, ratio_rows, mult):
-    """fp32 two-pass LayerNorm: the mean is a sum of C terms in <= 64 sequential fp32 additions (per-lane runs, then a
-    butterfly), so (x - mean) carries up to 2^-18 |mean| absolute error; relative to std that is 2^-18 |mean| / std, times
-    the output multiplier."""
-    return 2.0 ** -18 * (1 + ratio_rows) * mult
 
 
 @pytest.mark.parametrize("ratio", [0, 4, 32, 128])
