@@ -1,6 +1,10 @@
 """Sampling-loop benchmark: the S = 25 SA-Solver loop (scripts/inference.py:119-133's call) next to the 20-step DPM-Solver++
 loop (:102-118), eager and as one CUDA graph, around the full PixArt-Sigma-XL/2 denoiser at the c3 shapes of bench.py
 (1024px, 4 images, forward batch 8 = CFG pairs, 300 caption tokens, synthetic bf16 weights built as bench.py builds them).
+The IDDPM loop (:89-101: `IDDPM("100").p_sample_loop(model.forward_with_cfg, ..., clip_denoised=False)`, cfg 4.5) is timed
+three ways on the same model: the torch loop (`p_sample_loop_progressive` driven to the end), and the native loop eager and
+as one CUDA graph (with the capture time); `iddpm_native_vs_glue_rel_err` compares the native and the torch loop's samples
+drawn from the same seed.
 
 For each loop: wall time of one whole sampling run (CUDA events around work that ends in a synchronise, after a warm-up run
 that also captures the graph), denoise-steps/s (images x evaluations / s), library kernel launches per evaluation (eager), and
@@ -8,7 +12,7 @@ the sampler overhead = loop time - evaluations x the time of one eager forward (
 within run-to-run noise that difference can come out slightly negative.  The card name,
 power limit and max SM clock are read (read-only) in the same run.  Prints one JSON line.
 
-    python bench_sampling.py [--reps 3] [--images 4] [--side 128]
+    python bench_sampling.py [--reps 3] [--images 4] [--side 128] [--iddpm-steps 100]
 """
 import argparse
 import json
@@ -56,10 +60,12 @@ def main():
     ap.add_argument("--images", type=int, default=4)
     ap.add_argument("--side", type=int, default=128, help="latent side (128 = 1024px)")
     ap.add_argument("--depth", type=int, default=28)
+    ap.add_argument("--iddpm-steps", type=int, default=100, help="IDDPM respacing (scripts/inference.py's default: 100)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_sampling.py measures on the GPU; no CUDA device found")
     from pixart_sigma_b200 import PixArtMS, SASolverSampler, lib
+    from pixart_sigma_b200.iddpm import IDDPM
     from pixart_sigma_b200.sampler import DPMS
 
     dev = torch.device("cuda")
@@ -115,6 +121,40 @@ def main():
                     "evaluations": evals, "ms": round(ms, 2), "denoise_steps_per_s": round(imgs * evals / (ms / 1000.0), 3),
                     "launches_per_step": launches, "overhead_ms": round(ms - evals * fwd_ms, 2),
                     "overhead_ms_per_step": round((ms - evals * fwd_ms) / evals, 3)}
+
+        # IDDPM as scripts/inference.py:89-101 runs it: the n latents repeated to the 2n CFG batch, y = [caption ; null]
+        steps = args.iddpm_steps
+        iddpm = IDDPM(str(steps))
+        z2 = z.repeat(2, 1, 1, 1)
+        ikw = dict(y=torch.cat([cond, null]), cfg_scale=4.5, data_info=None, mask=mask)
+        icall = dict(clip_denoised=False, model_kwargs=ikw, device=dev)
+
+        def glue():
+            for out in iddpm.p_sample_loop_progressive(model.forward_with_cfg, z2.shape, z2, **icall):
+                pass
+            return out["sample"]
+        iloops = {"glue": glue,
+                  "eager": lambda: iddpm.p_sample_loop(model.forward_with_cfg, z2.shape, z2, **icall),
+                  "graph": lambda: iddpm.p_sample_loop(model.forward_with_cfg, z2.shape, z2, cuda_graph=True, **icall)}
+        samples = {}
+        for form, run in iloops.items():
+            torch.cuda.manual_seed(5)
+            samples[form] = run()                                             # warm-up (and capture), seeded
+            n0 = lib.launch_count()
+            if form != "graph":
+                run()
+                torch.cuda.synchronize()
+            launches = (lib.launch_count() - n0) / steps if form != "graph" else None
+            ms = timed_ms(run, args.reps)
+            entry = {"evaluations": steps, "ms": round(ms, 2), "denoise_steps_per_s": round(imgs * steps / (ms / 1000.0), 3),
+                     "launches_per_step": launches, "overhead_ms": round(ms - steps * fwd_ms, 2),
+                     "overhead_ms_per_step": round((ms - steps * fwd_ms) / steps, 3)}
+            if form == "graph":
+                entry["capture_s"] = round(iddpm.last_capture_s, 2)
+            res[f"iddpm_s{steps}_{form}"] = entry
+        ref = samples["glue"].double()
+        res["iddpm_native_vs_glue_rel_err"] = {
+            form: float((samples[form].double() - ref).norm() / ref.norm()) for form in ("eager", "graph")}
     res["forward"]["ms"] = round(fwd_ms, 2)
     print(json.dumps(res))
 

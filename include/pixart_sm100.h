@@ -32,6 +32,7 @@ extern "C" {
 
 #define PXA_DTYPE_BF16 0
 #define PXA_DTYPE_F32 1
+#define PXA_DTYPE_F16 2      /* accepted only where an entry point says so (pxa_iddpm_step) */
 
 int pxa_version(void);
 const char* pxa_last_error(void);
@@ -469,6 +470,39 @@ typedef struct PxaSaStepArgs {
   float p_x, p_m0, p_m1, p_noise;
 } PxaSaStepArgs;
 int pxa_sa_solver_step(const PxaSaStepArgs* args, void* stream);
+
+/* ------------------------------------------------------------------------------------ IDDPM ancestral step
+ * One fused elementwise pass per step of the IDDPM sampling loop the reference runs in PyTorch as scripts/inference.py:89-101
+ * calls it (`IDDPM(str(steps)).p_sample_loop(model.forward_with_cfg, ...)`): p_mean_variance with LEARNED_RANGE variance and
+ * EPSILON prediction (diffusion/model/gaussian_diffusion.py:280-361), p_sample (:405-446), and the CFG mix of
+ * forward_with_cfg (diffusion/model/nets/PixArtMS.py:221-234).  Per element of row r (fp32 arithmetic):
+ *     eps      = model_out[r, c]                      c = 0..3; guided and c < 3: eps_u + cfg_scale (eps_c - eps_u), the
+ *                                                     same mixed value for both rows of the pair (channel 3 stays the row's own)
+ *     frac     = (model_out[r, 4 + c] + 1) / 2        (the row's own variance channel)
+ *     logvar   = frac * log_beta + (1 - frac) * post_logvar
+ *     pred_x0  = sqrt_recip_ac * img - sqrt_recipm1_ac * eps,   clamped to [-1, 1] when clip
+ *     img     <- post_c1 * pred_x0 + post_c2 * img  (+ exp(0.5 * logvar) * noise when noise != NULL, i.e. t != 0)
+ * Guided: N = 2n rows ordered [cond (n) ; uncond (n)] (inference.py:93, the reverse of the DPM / SA steps), both halves of
+ * img are updated, and next_in receives the next model input [img[:n] ; img[:n]] (forward_with_cfg's cat([half, half])).
+ * Unguided: N = n rows used as they are; next_in is not written (the next model input is img itself) and may be NULL.
+ * The host computes every scalar once per step, as the fp64 tables rounded to fp32 (`_extract_into_tensor`).
+ * model_out: [N, 8, hw] in out_dtype (fp32, bf16 or fp16), row r at r * out_batch_stride, channel c at c * hw.  img, noise,
+ * next_in: fp32 [N, 4, hw] contiguous, 4-byte aligned.  Any hw.  HBM-bound: 16 (fp32 out) / 12 (bf16 / fp16 out) + 4 (noise)
+ * + 4 (guided: next_in) algorithmic bytes per latent element.
+ */
+typedef struct PxaIddpmStepArgs {
+  const void* model_out;    /* [N, 8, hw], dtype out_dtype                                          */
+  float* img;               /* fp32 [N, 4, hw] in/out: x_t -> x_{t-1}                                */
+  const float* noise;       /* fp32 [N, 4, hw], or NULL at t == 0                                    */
+  float* next_in;           /* fp32 [N, 4, hw] out (guided), ignored when unguided                   */
+  int64_t out_batch_stride; /* elements                                                              */
+  int32_t n, hw;            /* n images: N = 2n rows guided, n unguided                              */
+  int32_t out_dtype;        /* PXA_DTYPE_F32, PXA_DTYPE_BF16 or PXA_DTYPE_F16                        */
+  int32_t guided;           /* 1: CFG pairs [cond ; uncond], cfg_scale used; 0: rows as they are     */
+  int32_t clip;             /* 1: clamp pred_x0 to [-1, 1] (clip_denoised)                           */
+  float cfg_scale, sqrt_recip_ac, sqrt_recipm1_ac, post_c1, post_c2, log_beta, post_logvar;
+} PxaIddpmStepArgs;
+int pxa_iddpm_step(const PxaIddpmStepArgs* args, void* stream);
 
 /* ------------------------------------------------------------------------------------ LCM sampler step
  * One step of the reference's 4-step LCM sampler (`LCMScheduler.step`, diffusion/lcm_scheduler.py:310-410, epsilon

@@ -7,6 +7,8 @@ Only what the path `PixArtMS.forward -> 28 x PixArtMSBlock.forward` needs:
   sampler.py DPM-Solver++ loop around the path (mirror of the reference's `diffusion.DPMS`), fused step kernel + CUDA graph
   sa_sampler.py  SA-Solver loop (mirror of the reference's `diffusion.SASolverSampler`), fused predictor-corrector step
              kernel + CUDA graph
+  iddpm.py   IDDPM ancestral loop (mirror of the reference's `diffusion.IDDPM`), fused CFG-mix + ancestral step kernel + CUDA
+             graph on CUDA latents, the torch restatement on CPU
   lcm.py     LCM: the few-step sampler (mirror of the reference's `LCMScheduler` loop) and consistency distillation with a
              fused flat EMA update
   dmd.py     DMD: distribution-matching distillation to a one-step generator (fused loss kernel) and one-step sampling

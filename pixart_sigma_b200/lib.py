@@ -18,7 +18,7 @@ EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_RESIDUAL = 0, 1, 2
 EPI_BIAS_GELU_AUX, EPI_MUL_DGELU = 3, 4      # MLP training fusions (include/pixart_sm100.h)
 EPI_LN_BIAS, EPI_LN_BIAS_GELU = 5, 6         # fused LayerNorm-modulate consumer epilogues
 LN_STAT_PARTS = 8
-DTYPE_BF16, DTYPE_F32 = 0, 1
+DTYPE_BF16, DTYPE_F32, DTYPE_F16 = 0, 1, 2    # DTYPE_F16: pxa_iddpm_step only
 
 
 class PxaError(RuntimeError):
@@ -145,6 +145,14 @@ class SaStepArgs(C.Structure):
                 ("p_x", C.c_float), ("p_m0", C.c_float), ("p_m1", C.c_float), ("p_noise", C.c_float)]
 
 
+class IddpmStepArgs(C.Structure):
+    _fields_ = [("model_out", C.c_void_p), ("img", C.c_void_p), ("noise", C.c_void_p), ("next_in", C.c_void_p),
+                ("out_batch_stride", C.c_int64), ("n", C.c_int32), ("hw", C.c_int32), ("out_dtype", C.c_int32),
+                ("guided", C.c_int32), ("clip", C.c_int32), ("cfg_scale", C.c_float), ("sqrt_recip_ac", C.c_float),
+                ("sqrt_recipm1_ac", C.c_float), ("post_c1", C.c_float), ("post_c2", C.c_float), ("log_beta", C.c_float),
+                ("post_logvar", C.c_float)]
+
+
 class LcmStepArgs(C.Structure):
     _fields_ = [("model_out", C.c_void_p), ("x", C.c_void_p), ("noise", C.c_void_p), ("denoised", C.c_void_p),
                 ("x_next", C.c_void_p), ("out_batch_stride", C.c_int64), ("n", C.c_int32), ("hw", C.c_int32),
@@ -232,7 +240,7 @@ EXPORTS = ("pxa_transpose_bf16", "pxa_gelu_tanh_bf16", "pxa_gate_residual_fwd", 
            "pxa_version", "pxa_last_error", "pxa_launch_count", "pxa_gemm_bf16", "pxa_ln_modulate",
            "pxa_flash_attn_d72_bf16", "pxa_kv_compress_conv2_ln", "pxa_conv3x3_nhwc_bf16", "pxa_dpm_solver_pp_step",
            "pxa_ln_prepare", "pxa_layernorm_affine_bf16", "pxa_groupnorm_silu_nhwc_bf16", "pxa_adamw_flat", "pxa_mlp_fused_bf16",
-           "pxa_rmsnorm_bf16", "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step",
+           "pxa_rmsnorm_bf16", "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step", "pxa_iddpm_step",
            "pxa_grad_clip_flat", "pxa_came_workspace_bytes", "pxa_came_flat",
            "pxa_lcm_step", "pxa_lcm_teacher_target", "pxa_lcm_consistency_loss", "pxa_ema_flat",
            "pxa_dmd_loss", "pxa_gemm_lora_bf16")
@@ -255,7 +263,8 @@ def load() -> C.CDLL:
                              ("pxa_conv3x3_nhwc_bf16", Conv3x3Args), ("pxa_dpm_solver_pp_step", DpmStepArgs),
                              ("pxa_ln_prepare", LnPrepareArgs), ("pxa_adamw_flat", AdamWArgs),
                              ("pxa_mlp_fused_bf16", MlpArgs), ("pxa_t5_attn_d64_bf16", T5AttnArgs),
-                             ("pxa_sa_solver_step", SaStepArgs), ("pxa_grad_clip_flat", GradClipArgs),
+                             ("pxa_sa_solver_step", SaStepArgs), ("pxa_iddpm_step", IddpmStepArgs),
+                             ("pxa_grad_clip_flat", GradClipArgs),
                              ("pxa_came_flat", CameArgs), ("pxa_lcm_step", LcmStepArgs),
                              ("pxa_lcm_teacher_target", LcmTeacherArgs), ("pxa_lcm_consistency_loss", LcmLossArgs),
                              ("pxa_ema_flat", EmaArgs), ("pxa_dmd_loss", DmdLossArgs)):
@@ -636,6 +645,33 @@ def sa_solver_step(model_out: torch.Tensor, x: torch.Tensor, x_pred: torch.Tenso
                       p_m1=p_m1, p_noise=p_noise)
     _check(load().pxa_sa_solver_step(C.byref(args), _stream()), "pxa_sa_solver_step")
     return x_pred
+
+
+_IDDPM_DTYPES = {torch.float32: DTYPE_F32, torch.bfloat16: DTYPE_BF16, torch.float16: DTYPE_F16}
+
+
+def iddpm_step(model_out: torch.Tensor, img: torch.Tensor, noise: Optional[torch.Tensor], next_in: Optional[torch.Tensor], *,
+               guided: bool, clip: bool, cfg_scale: float, sqrt_recip_ac: float, sqrt_recipm1_ac: float, post_c1: float,
+               post_c2: float, log_beta: float, post_logvar: float) -> torch.Tensor:
+    """One IDDPM ancestral step, in place on img (include/pixart_sm100.h: pxa_iddpm_step); returns img.  model_out: the
+    learn-sigma output (N, 8, h, w) in fp32, bf16 or fp16 with dense (h, w) planes; guided: N = 2n rows [cond ; uncond], the
+    first three eps channels mixed with cfg_scale, and next_in receives [img[:n] ; img[:n]].  img, noise, next_in: fp32
+    (N, 4, h, w) contiguous; noise None at t = 0, next_in None when unguided."""
+    lat = [t for t in (img, noise, next_in) if t is not None]
+    assert model_out.is_cuda and all(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() for t in lat)
+    assert img.dim() == 4 and img.shape[1] == 4 and all(t.shape == img.shape for t in lat)
+    assert next_in is not None or not guided
+    N, _, h, w = img.shape
+    assert not guided or N % 2 == 0, "guided: the batch is CFG pairs [cond ; uncond]"
+    assert model_out.dtype in _IDDPM_DTYPES and tuple(model_out.shape) == (N, 8, h, w)
+    assert model_out.stride(3) == 1 and model_out.stride(2) == w and model_out.stride(1) == h * w, "model_out: (.., h, w) planes must be dense"
+    args = IddpmStepArgs(model_out=_ptr(model_out), img=_ptr(img), noise=_ptr(noise), next_in=_ptr(next_in),
+                         out_batch_stride=model_out.stride(0), n=N // 2 if guided else N, hw=h * w,
+                         out_dtype=_IDDPM_DTYPES[model_out.dtype], guided=int(bool(guided)), clip=int(bool(clip)),
+                         cfg_scale=cfg_scale, sqrt_recip_ac=sqrt_recip_ac, sqrt_recipm1_ac=sqrt_recipm1_ac, post_c1=post_c1,
+                         post_c2=post_c2, log_beta=log_beta, post_logvar=post_logvar)
+    _check(load().pxa_iddpm_step(C.byref(args), _stream()), "pxa_iddpm_step")
+    return img
 
 
 def _lcm_out(t: torch.Tensor, rows: int, h: int, w: int, what: str) -> None:

@@ -927,10 +927,12 @@ def install_into_reference() -> bool:
     nets.PixArtBlock = PixArtBlock
     try:                                                   # the samplers the inference script imports from `diffusion`
         import diffusion
+        from .iddpm import IDDPM
         from .sa_sampler import SASolverSampler
         from .sampler import DPMS
         diffusion.DPMS = DPMS
         diffusion.SASolverSampler = SASolverSampler
+        diffusion.IDDPM = IDDPM
     except Exception:
         pass
     return True
