@@ -411,6 +411,26 @@ typedef struct PxaConv3x3Args {
 } PxaConv3x3Args;
 int pxa_conv3x3_nhwc_bf16(const PxaConv3x3Args* args, void* stream);
 
+/* ------------------------------------------------------------------------------------ VAE output head to uint8 pixels
+ * The decoder's conv_out (Cin -> 3 channels, 3x3, zero padding 1) on the NHWC bf16 output of conv_norm_out + SiLU, then
+ * torchvision.utils.save_image's arithmetic (normalize=True, value_range=(-1, 1); call site scripts/inference.py:136-143):
+ *     y[b,i,j,o] = bias[o] + sum_{dy,dx,c} w[o, dy, dx, c] * x[b, i+dy-1, j+dx-1, c]        (fp32 accumulation)
+ *     u8         = trunc(clamp(((clamp(y, -1, 1) + 1) / 2) * 255 + 0.5, 0, 255))         (op by op in fp32, round to nearest)
+ * x is addressed as x[b * x_sb + i * x_sh + j * x_sw + c] (elements; a channels_last tensor or a view with padded strides).
+ * Requirements: B, H, W >= 1 (any H, W); Cin a multiple of 8; x 16-byte aligned with strides multiples of 8 elements.
+ * Direct convolution on CUDA cores with an 8 x 32-pixel tile plus one-pixel halo staged in shared memory.
+ */
+typedef struct PxaVaeOutArgs {
+  const void* x;        /* bf16 [B, H, W, Cin] with the strides below                                          */
+  const void* w;        /* bf16 [3, 3, 3, Cin] contiguous = checkpoint weight [3, Cin, 3, 3] permuted            */
+  const float* bias;    /* fp32 [3]                                                                            */
+  uint8_t* out_u8;      /* uint8 [B, H, W, 3] contiguous                                                       */
+  float* out_f32;       /* fp32 [B, H, W, 3] contiguous (y before the conversion), or NULL                     */
+  int64_t x_sb, x_sh, x_sw;
+  int32_t B, H, W, Cin;
+} PxaVaeOutArgs;
+int pxa_vae_out_u8(const PxaVaeOutArgs* args, void* stream);
+
 /* ------------------------------------------------------------------------------------ DPM-Solver++ sampler step
  * One fused elementwise pass per sampling step of the multistep DPM-Solver++ (2M) loop the reference runs in PyTorch
  * (diffusion/model/dpm_solver.py: CFG combine :326-332, data prediction :435-444, first-order update :565-577,

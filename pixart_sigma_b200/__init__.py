@@ -17,6 +17,7 @@ Only what the path `PixArtMS.forward -> 28 x PixArtMSBlock.forward` needs:
   parallel.py  batch-sharded inference replicas; bucketed gradient all-reduce for data-parallel training
   vae.py / t5.py  the callers either side of the path on the same kernels: SDXL-VAE (diffusers' AutoencoderKL layout) and the
              T5-v1.1-XXL caption encoder (transformers' T5EncoderModel layout)
+  pipeline.py / generate.py  text to image on these modules (the reference's scripts/inference.py flow) and its CLI
   build.py   in-tree nvcc build
 """
 from .model import (MODELS, PixArt, PixArt_XL_2, PixArtBlock, PixArtMS, PixArtMS_XL_2, PixArtMSBlock,  # noqa: F401

@@ -192,7 +192,9 @@ class IDDPMSampler:
         """(steps, rows) int64 mapped timesteps of every step on `device`: one upload, kept for later calls."""
         key = (str(device), rows)
         if key not in self._tmaps:
-            self._tmaps[key] = torch.tensor([[st["map_t"]] * rows for st in self.plan()], dtype=torch.int64).to(device)
+            tab = torch.tensor([[st["map_t"]] * rows for st in self.plan()], dtype=torch.int64)
+            # through pinned memory: the upload does not wait for the device
+            self._tmaps[key] = tab.pin_memory().to(device, non_blocking=True) if device.type == "cuda" else tab.to(device)
         return self._tmaps[key]
 
     # ---- native loop: device side

@@ -129,6 +129,12 @@ class Conv3x3Args(C.Structure):
                 ("B", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("Cin", C.c_int32), ("Cout", C.c_int32)]
 
 
+class VaeOutArgs(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("w", C.c_void_p), ("bias", C.c_void_p), ("out_u8", C.c_void_p), ("out_f32", C.c_void_p),
+                ("x_sb", C.c_int64), ("x_sh", C.c_int64), ("x_sw", C.c_int64), ("B", C.c_int32), ("H", C.c_int32), ("W", C.c_int32),
+                ("Cin", C.c_int32)]
+
+
 class DpmStepArgs(C.Structure):
     _fields_ = [("model_out", C.c_void_p), ("x", C.c_void_p), ("x0_prev", C.c_void_p), ("out_batch_stride", C.c_int64),
                 ("n", C.c_int32), ("hw", C.c_int32), ("out_dtype", C.c_int32),
@@ -243,7 +249,7 @@ EXPORTS = ("pxa_transpose_bf16", "pxa_gelu_tanh_bf16", "pxa_gate_residual_fwd", 
            "pxa_rmsnorm_bf16", "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step", "pxa_iddpm_step",
            "pxa_grad_clip_flat", "pxa_came_workspace_bytes", "pxa_came_flat",
            "pxa_lcm_step", "pxa_lcm_teacher_target", "pxa_lcm_consistency_loss", "pxa_ema_flat",
-           "pxa_dmd_loss", "pxa_gemm_lora_bf16")
+           "pxa_dmd_loss", "pxa_gemm_lora_bf16", "pxa_vae_out_u8")
 
 _lib = None
 
@@ -267,7 +273,7 @@ def load() -> C.CDLL:
                              ("pxa_grad_clip_flat", GradClipArgs),
                              ("pxa_came_flat", CameArgs), ("pxa_lcm_step", LcmStepArgs),
                              ("pxa_lcm_teacher_target", LcmTeacherArgs), ("pxa_lcm_consistency_loss", LcmLossArgs),
-                             ("pxa_ema_flat", EmaArgs), ("pxa_dmd_loss", DmdLossArgs)):
+                             ("pxa_ema_flat", EmaArgs), ("pxa_dmd_loss", DmdLossArgs), ("pxa_vae_out_u8", VaeOutArgs)):
             fn = getattr(lib, name)
             fn.restype = C.c_int
             fn.argtypes = [C.POINTER(struct), C.c_void_p]
@@ -500,6 +506,31 @@ def conv3x3_nhwc(x: torch.Tensor, w_packed: torch.Tensor, bias: Optional[torch.T
                        Cin=Cin, Cout=Cout)
     _check(load().pxa_conv3x3_nhwc_bf16(C.byref(args), _stream()), "pxa_conv3x3_nhwc_bf16")
     return out
+
+
+def vae_out_u8(x: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor, out_u8: torch.Tensor,
+               out_f32: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The VAE decoder's conv_out (3x3, pad 1, Cin -> 3) and save_image's uint8 conversion in one pass (pxa_vae_out_u8).
+    x: bf16 (B, H, W, Cin) with unit channel stride and the other strides multiples of 8 (a channels_last tensor or a padded
+    view); w_packed: bf16 (3, 3, 3, Cin) contiguous; bias: fp32 (3,); out_u8: uint8 (B, H, W, 3) contiguous; out_f32: the fp32
+    convolution output (B, H, W, 3) contiguous, or None."""
+    if not (x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.stride(3) == 1):
+        raise PxaError("vae_out_u8: x must be a bf16 CUDA tensor (B, H, W, Cin) with unit channel stride")
+    B, H, W, Cin = x.shape
+    if not (w_packed.dtype == torch.bfloat16 and w_packed.is_contiguous() and tuple(w_packed.shape) == (3, 3, 3, Cin)):
+        raise PxaError(f"vae_out_u8: w_packed must be contiguous bf16 (3, 3, 3, {Cin})")
+    if not (bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == 3):
+        raise PxaError("vae_out_u8: bias must be 3 contiguous fp32 values")
+    if not (out_u8.dtype == torch.uint8 and out_u8.is_contiguous() and tuple(out_u8.shape) == (B, H, W, 3)):
+        raise PxaError(f"vae_out_u8: out_u8 must be contiguous uint8 ({B}, {H}, {W}, 3)")
+    if out_f32 is not None and not (out_f32.dtype == torch.float32 and out_f32.is_contiguous() and tuple(out_f32.shape) == (B, H, W, 3)):
+        raise PxaError(f"vae_out_u8: out_f32 must be contiguous fp32 ({B}, {H}, {W}, 3)")
+    if not all(t.device == x.device for t in (w_packed, bias, out_u8) + ((out_f32,) if out_f32 is not None else ())):
+        raise PxaError("vae_out_u8: all tensors must be on the same CUDA device")
+    args = VaeOutArgs(x=_ptr(x), w=_ptr(w_packed), bias=_ptr(bias), out_u8=_ptr(out_u8), out_f32=_ptr(out_f32), x_sb=x.stride(0),
+                      x_sh=x.stride(1), x_sw=x.stride(2), B=B, H=H, W=W, Cin=Cin)
+    _check(load().pxa_vae_out_u8(C.byref(args), _stream()), "pxa_vae_out_u8")
+    return out_u8
 
 
 def _env_int(name: str, default: int) -> int:

@@ -590,7 +590,8 @@ def _pos_embed_fp32(C: int, h: int, w: int, pe_interpolation: float, base_size: 
         aw = np.tile(pos_w[None, :], (h, 1)).reshape(-1)[:, None] * omega[None]     # w varies fastest
         ah = np.repeat(pos_h, w)[:, None] * omega[None]
         full = np.concatenate([np.sin(aw), np.cos(aw), np.sin(ah), np.cos(ah)], axis=1)
-        tab = torch.from_numpy(full).to(torch.float32).to(device)
+        tab = torch.from_numpy(full).to(torch.float32)
+        tab = tab.pin_memory().to(device, non_blocking=True) if torch.device(device).type == "cuda" else tab.to(device)
         _POS_CACHE[key] = tab
     return tab
 

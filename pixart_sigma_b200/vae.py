@@ -249,14 +249,35 @@ class VaeDecoder(nn.Module):
         self.conv_out = nn.Conv2d(ch[0], cfg["out_channels"], 3, padding=1)
         self._cache = {}
 
-    @torch.no_grad()
-    def forward(self, z: torch.Tensor) -> torch.Tensor:
+    def _trunk(self, z: torch.Tensor) -> torch.Tensor:
+        """conv_in -> mid block -> up blocks: everything before conv_norm_out."""
         _need_kernels(z, self.conv_in.weight, "VaeDecoder")
         x = F.conv2d(z.to(torch.bfloat16), self.conv_in.weight, self.conv_in.bias, padding=1).contiguous(memory_format=torch.channels_last)
         x = self.mid_block(x)
         for blk in self.up_blocks:
             x = blk(x)
-        return _norm_act_conv(self.conv_norm_out, self.conv_out, x, self._cache)
+        return x
+
+    @torch.no_grad()
+    def forward(self, z: torch.Tensor) -> torch.Tensor:
+        return _norm_act_conv(self.conv_norm_out, self.conv_out, self._trunk(z), self._cache)
+
+    @torch.no_grad()
+    def forward_uint8(self, z: torch.Tensor, return_float: bool = False):
+        """z (B, 4, h, w) -> (uint8 pixels (B, H, W, 3), conv_out's fp32 output (B, H, W, 3) or None): conv_norm_out + SiLU on
+        the GroupNorm kernel, then conv_out and save_image's conversion in one `pxa_vae_out_u8` pass."""
+        xh = _nhwc(self._trunk(z))
+        norm, conv = self.conv_norm_out, self.conv_out
+        h = lib.groupnorm_silu_nhwc(xh, norm.weight, norm.bias, torch.empty_like(xh), groups=norm.num_groups, eps=norm.eps, silu=True)
+        key = (conv.weight._version, conv.weight.data_ptr(), conv.bias._version, conv.bias.data_ptr())
+        if self._cache.get("u8_key") != key:
+            self._cache["u8_key"] = key
+            self._cache["u8_w"] = conv.weight.detach().to(torch.bfloat16).permute(0, 2, 3, 1).contiguous()
+            self._cache["u8_b"] = conv.bias.detach().float().contiguous()
+        B, H, W, _ = h.shape
+        out = torch.empty(B, H, W, 3, dtype=torch.uint8, device=h.device)
+        y = torch.empty(B, H, W, 3, dtype=torch.float32, device=h.device) if return_float else None
+        return lib.vae_out_u8(h, self._cache["u8_w"], self._cache["u8_b"], out, y), y
 
 
 class VaeEncoder(nn.Module):
@@ -328,6 +349,18 @@ class AutoencoderKL(nn.Module):
         z = F.conv2d(z.to(self.post_quant_conv.weight.dtype), self.post_quant_conv.weight, self.post_quant_conv.bias)
         img = self.decoder(z)
         return _Sample(img) if return_dict else (img,)
+
+    @torch.no_grad()
+    def decode_to_uint8(self, z: torch.Tensor, return_float: bool = False):
+        """`decode(z).sample` written straight to image bytes: uint8 (B, H, W, 3) on the device, equal to what
+        torchvision's `save_image(img, normalize=True, value_range=(-1, 1))` makes of the decoded image (before the JPEG
+        encoder).  The decoder's conv_out and the conversion run as one kernel (`pxa_vae_out_u8`).  With return_float, also
+        returns conv_out's fp32 output as a (B, 3, H, W) view of an NHWC tensor."""
+        z = F.conv2d(z.to(self.post_quant_conv.weight.dtype), self.post_quant_conv.weight, self.post_quant_conv.bias)
+        if self.decoder.conv_out.out_channels != 3:
+            raise ValueError("decode_to_uint8 needs a decoder with 3 output channels")
+        u8, y = self.decoder.forward_uint8(z, return_float)
+        return (u8, y.permute(0, 3, 1, 2)) if return_float else u8
 
     @torch.no_grad()
     def encode(self, img: torch.Tensor, return_dict: bool = True):
