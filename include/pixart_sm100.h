@@ -70,9 +70,6 @@ uint64_t pxa_launch_count(void);
 #define PXA_EPI_LN_BIAS_GELU 6  /* out = gelu_tanh(rstd*(acc - mu*u) + v)                                                   */
 #define PXA_LN_STAT_PARTS 8     /* row statistics are kept as 8 partial (sum x, sum x^2) pairs per row: fp32 [M][8][2]      */
 
-/* The structure keeps the layout it had when the library offered several kernel forms per call.  On sm_90 there is one GEMM
- * kernel (128 x BN tiles on one CTA), so `cta_pair`, `res_epilogue`, `epi_warps` and `debug_trace` are validated where noted and
- * otherwise ignored. */
 typedef struct PxaGemmArgs {
   const void* a;        /* bf16 [M, K], row stride lda (elements)                                   */
   const void* w;        /* bf16 [N, K], row stride ldw (elements)                                   */
@@ -89,8 +86,6 @@ typedef struct PxaGemmArgs {
   int32_t out_dtype;    /* PXA_DTYPE_*          */
   int32_t block_n;      /* 0 = auto (192 when it divides N, else 128); or 128 / 192 / 256 (fp32 out: 256 runs as 128) */
   int32_t max_ctas;     /* 0 = one CTA per SM; >0 caps the persistent grid (tests)                  */
-  int32_t cta_pair;     /* (ignored, see above; must be 0, 1 or 2) */
-  int64_t* debug_trace; /* (ignored) */
   int32_t operands_mn_major; /* 1: weight-gradient form out[M, N] += A^T . W with a = [K, M] (row stride lda) and
                                 w = [K, N] (row stride ldw), i.e. the contraction runs over the ROWS of both operands
                                 (dW = dY^T X straight from the activations' natural layouts; no transposes).  Requires
@@ -111,8 +106,6 @@ typedef struct PxaGemmArgs {
   int64_t ln_uv_batch_stride;
   int32_t ln_dim;           /* row length C of x the statistics were taken over                                              */
   float ln_eps;
-  int32_t res_epilogue;     /* (ignored; must be 0, 1 or 2) */
-  int32_t epi_warps;        /* (ignored) */
   int32_t reverse_tiles;    /* 1: visit the output tiles from the LAST row block to the first.  A GEMM whose A operand was
                                written front to back by the previous kernel (mlp.fc2 after mlp.fc1) then starts on the rows
                                that are still in the 50 MB L2 instead of the ones already evicted to HBM                   */
@@ -136,38 +129,6 @@ typedef struct PxaGemmTail {
   int32_t lda_tail, ldw_tail;
 } PxaGemmTail;
 int pxa_gemm_lora_bf16(const PxaGemmArgs* args, const PxaGemmTail* tail, void* stream);
-
-/* ------------------------------------------------------------------------------------------- fused Mlp
- * x32[r, :] += gate[b, :] * ( gelu_tanh(x[r, :] W1^T + b1) W2^T + b2 )        b = r / rows_per_batch
- * The timm Mlp of PixArtMSBlock with its gate and residual (PixArtMS.py:67,77), run in groups of `group` 256-row panels: per group
- * one fc1 + GELU launch and one fc2 + gate + residual launch of the GEMM kernel, back to back on the stream, so that the group's
- * [rows, N1] hidden activations sit in a slot of a small ring (hidden_ws) that lives in L2 instead of streaming through HBM
- * (mlp_sm90.cu; 2 * ceil(M / (256 group)) launches, not one kernel).  x = the normalised, modulated bf16 activations
- * (pxa_ln_modulate output); x32 = the fp32 residual stream, updated in place.
- */
-typedef struct PxaMlpArgs {
-  const void* x;         /* bf16 [M, K1], row stride ldx                                   */
-  const void* w1;        /* bf16 [N1, K1] (mlp.fc1.weight), row stride ldw1                 */
-  const void* b1;        /* bf16 [N1] or NULL                                              */
-  const void* w2;        /* bf16 [N2, N1] (mlp.fc2.weight), row stride ldw2                 */
-  const void* b2;        /* bf16 [N2] or NULL                                              */
-  float* x32;            /* fp32 [M, N2], row stride ldo: residual stream, updated in place */
-  const float* gate;     /* fp32 (b, n) at gate[b*gate_batch_stride + n], or NULL           */
-  int64_t gate_batch_stride;
-  void* hidden_ws;       /* bf16 scratch, >= ring * group * 256 * N1 elements               */
-  int64_t hidden_ws_bytes;
-  void* flags_ws;        /* unused (may be NULL); kept for binary compatibility                                   */
-  int64_t flags_ws_bytes;
-  int32_t rows_per_batch;
-  int32_t M, K1, N1, N2; /* N1 % 256 == 0, N2 % 192 == 0                                   */
-  int32_t ldx, ldw1, ldw2, ldo;
-  int32_t group;         /* 256-row panels per group (0 = 4)                               */
-  int32_t ring;          /* groups held by hidden_ws (0 = 2): group g uses slot g % ring   */
-  int32_t max_ctas;      /* 0 = one CTA per SM; > 0 caps the persistent grid (tests)       */
-  int32_t lag;           /* unused */
-  int32_t k_splits;      /* unused */
-} PxaMlpArgs;
-int pxa_mlp_fused_bf16(const PxaMlpArgs* args, void* stream);
 
 /* ------------------------------------------------------------------------------------ LayerNorm + modulate
  * out[r,:] = LN(x[r,:]; eps, no affine) * (1 + scale[b,:]) + shift[b,:]  with b = r / rows_per_batch, bf16 out.
@@ -361,17 +322,14 @@ typedef struct PxaAttnArgs {
   int32_t B, H, Nq, Nk; /* Nk = max keys per sample (loop bound) */
   int32_t ldo;
   float scale;      /* softmax scale, 72^-0.5 */
-  int64_t* debug_trace; /* ignored (kept for binary compatibility) */
   float* lse;       /* optional fp32 [B, H, Nq]: log2-domain log-sum-exp of the scaled scores, the softmax statistic the
                        backward pass recomputes P from (training); NULL for inference                              */
   int32_t reverse_batch; /* 1: CTAs take the samples from the last to the first (same L2 argument as PxaGemmArgs.reverse_tiles:
                             the qkv rows of the last samples are the ones the QKV GEMM has just written)                   */
-  int32_t variant;  /* 0 or 2..7: accepted for compatibility; one kernel (attn_fwd.cuh) serves them all with identical arithmetic */
   int32_t p_precision; /* 0 = P rounded to bf16 before P V (up to 2^-8 relative; the default).
                           1 = `fp32_attention` semantics (PixArt_blocks.py:145-147: q / k / v and hence P kept in fp32): P enters
                               the tensor pipe as bf16 hi + lo terms (2^-17 relative), two P V products per 16 keys; logits,
-                              softmax and accumulation are fp32 in both modes.  Rejected together with variant 3.                  */
-  int32_t reserved0;   /* must be 0 */
+                              softmax and accumulation are fp32 in both modes.                                                   */
 } PxaAttnArgs;
 int pxa_flash_attn_d72_bf16(const PxaAttnArgs* args, void* stream);
 

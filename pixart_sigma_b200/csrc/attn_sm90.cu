@@ -16,9 +16,7 @@ extern "C" int pxa_flash_attn_d72_bf16(const PxaAttnArgs* args, void* stream) {
   if (reinterpret_cast<uintptr_t>(a.out) & 15) return fail(PXA_ERR_ALIGN, "out must be 16-byte aligned");
   if (a.H * kD > a.ldo) return fail(PXA_ERR_ARG, "ldo smaller than H*72");
   PXA_REQUIRE_SM90();
-  if (a.variant != 0 && (a.variant < 2 || a.variant > 7)) return fail(PXA_ERR_ARG, "variant must be 0 or 2..7");
   if (a.p_precision != 0 && a.p_precision != 1) return fail(PXA_ERR_ARG, "p_precision must be 0 (bf16 P) or 1 (bf16 hi + lo P)");
-  if (a.variant == 3 && a.p_precision) return fail(PXA_ERR_ARG, "variant 3 has no p_precision = 1 form");
   if (!(a.scale >= 0.f)) return fail(PXA_ERR_ARG, "scale must be >= 0");   // the kernel takes the row max on unscaled logits
   FaParams p = {};
   p.out = reinterpret_cast<__nv_bfloat16*>(a.out);

@@ -19,7 +19,6 @@ struct GemmParams {
   const float* gate;
   long long gate_batch_stride;
   int rows_per_batch;
-  int row_base;         // row r of this call is row row_base + r of the batch (sample = (row_base + r) / rows_per_batch)
   int M, N, K, ldo;
   int num_m_tiles, num_n_tiles;
   int k_splits;         // > 1: split-K over tiles (reduce-add epilogue only)
@@ -117,9 +116,9 @@ template <int BN> struct EpiRegs {
 
 template <int BN, bool kLn = false>
 PXA_DEVICE void load_epi_consts(EpiRegs<BN>& r, const GemmParams& p, int tid, int m0, int n0) {
-  const int b0 = (p.row_base + m0) / p.rows_per_batch;
+  const int b0 = m0 / p.rows_per_batch;
   const int last = (m0 + kBM - 1 < p.M ? m0 + kBM - 1 : p.M - 1);
-  const int b1 = (p.row_base + last) / p.rows_per_batch;
+  const int b1 = last / p.rows_per_batch;
 #pragma unroll
   for (int i = 0; i < EpiRegs<BN>::kCols; ++i) {
     const int col = n0 + tid + i * kNumEpiThreads;
@@ -138,7 +137,7 @@ PXA_DEVICE void load_epi_consts(EpiRegs<BN>& r, const GemmParams& p, int tid, in
       r.v[i][4] = (ok && p.aux_scale != nullptr) ? __ldg(p.aux_scale + (size_t)b1 * p.aux_scale_batch_stride + col) : 1.f;
     }
   }
-  r.row_split = (b0 + 1) * p.rows_per_batch - (p.row_base + m0);
+  r.row_split = (b0 + 1) * p.rows_per_batch - m0;
 }
 
 template <int BN>

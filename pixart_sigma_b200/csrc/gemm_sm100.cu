@@ -281,7 +281,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                 float2 gt = *reinterpret_cast<const float2*>((second ? cb->gate1 : cb->gate0) + tc);
                 if (per_row_gate)
                   gt = (grow < p.M && gcol < p.N)
-                           ? __ldg(reinterpret_cast<const float2*>(p.gate + (size_t)((p.row_base + grow) / p.rows_per_batch) *
+                           ? __ldg(reinterpret_cast<const float2*>(p.gate + (size_t)(grow / p.rows_per_batch) *
                                                                                  p.gate_batch_stride + gcol))
                            : make_float2(1.f, 1.f);
                 float2 r = make_float2(0.f, 0.f);
@@ -402,19 +402,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 
 
 // ------------------------------------------------------------------------------------------------- host
-// One GEMM call: the public arguments plus the row offset of the call within its batch (pxa_mlp_fused_bf16 runs the rows in
-// groups whose boundaries need not be sample boundaries: sample of row r = (row_base + r) / rows_per_batch).
-struct GemmCall : PxaGemmArgs {
-  int row_base = 0;
-};
-
 struct ConvGeom {
   int B, H, W, Cin, tile_w, tile_h;
   int Wp;          // virtual width of the M index (= W when W tiles; else W rounded up to 128, see GemmParams::conv_Wp)
 };
 
 template <int BN, int EPI, typename OutT, bool kConv = false, bool kMn = false, bool kTail = false>
-static int launch_gemm(const GemmCall& a, cudaStream_t stream, const ConvGeom* cg = nullptr, int k_splits = 1,
+static int launch_gemm(const PxaGemmArgs& a, cudaStream_t stream, const ConvGeom* cg = nullptr, int k_splits = 1,
                        const PxaGemmTail* tl = nullptr) {
   CUtensorMap ta, tw;
   if constexpr (kMn) {
@@ -487,7 +481,6 @@ static int launch_gemm(const GemmCall& a, cudaStream_t stream, const ConvGeom* c
   p.gate = a.gate;
   p.gate_batch_stride = a.gate_batch_stride;
   p.rows_per_batch = a.rows_per_batch > 0 ? a.rows_per_batch : a.M;
-  p.row_base = a.row_base;
   p.M = a.M; p.N = a.N; p.K = a.K; p.ldo = a.ldo;
   p.num_m_tiles = (a.M + kBM - 1) / kBM;
   p.num_n_tiles = (a.N + BN - 1) / BN;
@@ -513,7 +506,7 @@ static int launch_gemm(const GemmCall& a, cudaStream_t stream, const ConvGeom* c
 }
 
 template <int BN, bool kTail = false>
-static int dispatch_epi(const GemmCall& a, cudaStream_t s, const PxaGemmTail* tl = nullptr) {
+static int dispatch_epi(const PxaGemmArgs& a, cudaStream_t s, const PxaGemmTail* tl = nullptr) {
   switch (a.epilogue) {
     case PXA_EPI_BIAS:
       if (a.out_dtype != PXA_DTYPE_BF16) return fail(PXA_ERR_ARG, "EPI_BIAS writes bf16 only");
@@ -548,7 +541,7 @@ static int dispatch_epi(const GemmCall& a, cudaStream_t s, const PxaGemmTail* tl
 // the reduce-add epilogue, K split over tiles so that the persistent grid is evenly loaded (the layer shapes give
 // only 54 .. 216 output tiles against 132 SMs; each tile's K loop is thousands of blocks long).
 template <int BN>
-static int launch_wgrad(const GemmCall& a, cudaStream_t s) {
+static int launch_wgrad(const PxaGemmArgs& a, cudaStream_t s) {
   const int tiles = ((a.M + kBM - 1) / kBM) * ((a.N + BN - 1) / BN);
   const int num_kb = (a.K + kBK - 1) / kBK;
   int sms = device_info().sms;
@@ -566,7 +559,7 @@ static int launch_wgrad(const GemmCall& a, cudaStream_t s) {
 }
 
 template <int BN>
-static int dispatch_conv(const GemmCall& a, cudaStream_t s, const ConvGeom& cg) {
+static int dispatch_conv(const PxaGemmArgs& a, cudaStream_t s, const ConvGeom& cg) {
   if (a.epilogue == PXA_EPI_BIAS_RESIDUAL) return launch_gemm<BN, PXA_EPI_BIAS_RESIDUAL, __nv_bfloat16, true>(a, s, &cg);
   return launch_gemm<BN, PXA_EPI_BIAS, __nv_bfloat16, true>(a, s, &cg);
 }
@@ -599,7 +592,7 @@ extern "C" int pxa_conv3x3_nhwc_bf16(const PxaConv3x3Args* args, void* stream) {
        reinterpret_cast<uintptr_t>(c.bias) | reinterpret_cast<uintptr_t>(c.residual)) & 15)
     return fail(PXA_ERR_ALIGN, "pointers must be 16-byte aligned");
   PXA_REQUIRE_SM90();
-  GemmCall a = {};
+  PxaGemmArgs a = {};
   a.a = c.x; a.w = c.w; a.bias = c.bias; a.out = c.out; a.residual = c.residual;
   if ((long long)c.B * c.H * cg.Wp >= (1ll << 31)) return fail(PXA_ERR_ARG, "B x H x W too large");
   a.M = c.B * c.H * cg.Wp; a.N = c.Cout; a.K = 9 * c.Cin;
@@ -614,11 +607,9 @@ extern "C" int pxa_conv3x3_nhwc_bf16(const PxaConv3x3Args* args, void* stream) {
 }
 
 namespace pxa {
-static int gemm_impl(const PxaGemmArgs* args, int row_base, const PxaGemmTail* tl, void* stream) {
+static int gemm_impl(const PxaGemmArgs* args, const PxaGemmTail* tl, void* stream) {
   if (!args) return fail(PXA_ERR_ARG, "null args");
-  GemmCall a;
-  static_cast<PxaGemmArgs&>(a) = *args;
-  a.row_base = row_base;
+  const PxaGemmArgs& a = *args;
   if (!a.a || !a.w || !a.out) return fail(PXA_ERR_ARG, "null a / w / out");
   if (a.M <= 0 || a.N <= 0 || a.K <= 0) return fail(PXA_ERR_ARG, "bad shape M=%d N=%d K=%d", a.M, a.N, a.K);
   if ((a.N & 7) || (!a.operands_mn_major && (a.K & 7)) || (a.operands_mn_major && (a.M & 7)) || (a.lda & 7) ||
@@ -665,7 +656,6 @@ static int gemm_impl(const PxaGemmArgs* args, int row_base, const PxaGemmTail* t
   if (a.epilogue == PXA_EPI_BIAS_GELU_AUX && a.out_aux_bf16 == nullptr) return fail(PXA_ERR_ARG, "EPI_BIAS_GELU_AUX needs out_aux_bf16");
   if (a.epilogue == PXA_EPI_MUL_DGELU && (a.residual == nullptr || a.bias != nullptr))
     return fail(PXA_ERR_ARG, "EPI_MUL_DGELU needs the pre-activation in `residual` and no bias");
-  if (a.cta_pair < 0 || a.cta_pair > 2) return fail(PXA_ERR_ARG, "cta_pair must be 0, 1 or 2");
   // fused LayerNorm-modulate: consumer epilogues and the producer by-products of the fp32 residual epilogue
   const bool ln_epi = a.epilogue == PXA_EPI_LN_BIAS || a.epilogue == PXA_EPI_LN_BIAS_GELU;
   const int rpb = a.rows_per_batch > 0 ? a.rows_per_batch : a.M;
@@ -684,7 +674,6 @@ static int gemm_impl(const PxaGemmArgs* args, int row_base, const PxaGemmTail* t
   }
   if ((ln_epi || a.aux_scale) && rpb < kBM && a.M > rpb)
     return fail(PXA_ERR_ARG, "the fused LayerNorm-modulate needs rows_per_batch >= %d (a tile may span two samples at most)", kBM);
-  if (a.res_epilogue < 0 || a.res_epilogue > 2) return fail(PXA_ERR_ARG, "res_epilogue must be 0, 1 or 2");
   if (bn == 256 && a.out_dtype == PXA_DTYPE_F32) bn = 128;   // fp32 output tiles run at 128 columns (GemmCfg)
   // the tail instantiations spill at BN 256 and, with fp32 output, at BN 192: they run at 192 and 128 instead
   if (tl && bn == 256) bn = 192;
@@ -705,13 +694,11 @@ static int gemm_impl(const PxaGemmArgs* args, int row_base, const PxaGemmTail* t
     default: return fail(PXA_ERR_ARG, "block_n must be 0, 128, 192 or 256 (got %d)", bn);
   }
 }
-
-int gemm_bf16_rows(const PxaGemmArgs* args, int row_base, void* stream) { return gemm_impl(args, row_base, nullptr, stream); }
 }  // namespace pxa
 
-extern "C" int pxa_gemm_bf16(const PxaGemmArgs* args, void* stream) { return pxa::gemm_bf16_rows(args, 0, stream); }
+extern "C" int pxa_gemm_bf16(const PxaGemmArgs* args, void* stream) { return pxa::gemm_impl(args, nullptr, stream); }
 
 extern "C" int pxa_gemm_lora_bf16(const PxaGemmArgs* args, const PxaGemmTail* tail, void* stream) {
   if (!tail) return pxa::fail(PXA_ERR_ARG, "null tail");
-  return pxa::gemm_impl(args, 0, tail, stream);
+  return pxa::gemm_impl(args, tail, stream);
 }

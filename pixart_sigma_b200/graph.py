@@ -43,13 +43,13 @@ class GraphedForward:
                  data_info=None) -> torch.Tensor:
         require_lora_merged(self.model)           # a graph captured before an adapter was attached would ignore it
         dev = self._params[0].device
-        # The kernels read the parameters in place, but the forward also keeps derived copies (the row-stacked kv_linear weights
-        # of model._KvBatch, the fused-LN tables) that a captured graph cannot refresh: an in-place update or a re-assignment of
-        # any parameter (optimizer / EMA step, .to(dtype)) drops the captured graphs.
+        # The kernels read the parameters in place, but the fused-LN forward also keeps tables derived from them
+        # that a captured graph cannot refresh: an in-place update or a re-assignment of any parameter (optimizer / EMA step,
+        # .to(dtype)) drops the captured graphs.
         # (Without such copies -- the default configuration -- a replay reads the updated parameters in place and nothing is dropped.)
         wkey = (sum(p._version for p in self._params), self._params[0].data_ptr(), self._params[-1].data_ptr())
         if wkey != self._wkey:
-            derived = getattr(self.model, "_kv_batch", None) is not None or getattr(self.model, "_ln_fusion", None) is not None
+            derived = getattr(self.model, "_ln_fusion", None) is not None
             if self._wkey is not None and derived:
                 self._graphs.clear()
             self._wkey = wkey

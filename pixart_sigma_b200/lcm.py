@@ -265,8 +265,6 @@ def _inference_copy(model: torch.nn.Module) -> torch.nn.Module:
     for mod in m.modules():
         if "_ln_fusion" in mod.__dict__:
             mod.__dict__["_ln_fusion"] = None
-        if "_kv_batch" in mod.__dict__:
-            mod.__dict__["_kv_batch"] = None
         if isinstance(getattr(mod, "_ws", None), _Workspace):
             mod._ws = _Workspace()
     for p in m.parameters():
@@ -281,11 +279,10 @@ def _inference_copy(model: torch.nn.Module) -> torch.nn.Module:
 
 def _check_ema_forward(ema: torch.nn.Module, owner: str) -> None:
     """The EMA model's weights are rewritten by a kernel, which does not bump `_version`: the forward modes that keep
-    copies derived from the weights and keyed on `_version` (fused LayerNorm-modulate, batched kv_linear) would go stale."""
-    from . import model as _m
-    if getattr(ema, "fuse_ln_modulate", False) or (_m._KV_BATCH and len(getattr(ema, "blocks", ())) > 1):
-        raise RuntimeError(f"{owner}: the EMA model cannot use fuse_ln_modulate or PXA_KV_BATCH=1 (their derived weight "
-                           "copies are keyed on _version, which pxa_ema_flat does not bump)")
+    copies derived from the weights and keyed on `_version` (fused LayerNorm-modulate) would go stale."""
+    if getattr(ema, "fuse_ln_modulate", False):
+        raise RuntimeError(f"{owner}: the EMA model cannot use fuse_ln_modulate (its derived weight copies are keyed on "
+                           "_version, which pxa_ema_flat does not bump)")
 
 
 class FlatEMA:

@@ -32,12 +32,11 @@ class GemmArgs(C.Structure):
                 ("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32),
                 ("lda", C.c_int32), ("ldw", C.c_int32), ("ldo", C.c_int32),
                 ("epilogue", C.c_int32), ("out_dtype", C.c_int32), ("block_n", C.c_int32), ("max_ctas", C.c_int32),
-                ("cta_pair", C.c_int32), ("debug_trace", C.c_void_p), ("operands_mn_major", C.c_int32),
+                ("operands_mn_major", C.c_int32),
                 ("k_splits", C.c_int32), ("aux_is_branch", C.c_int32),
                 ("aux_scale", C.c_void_p), ("aux_scale_batch_stride", C.c_int64), ("row_stats_out", C.c_void_p),
                 ("ln_stats", C.c_void_p), ("ln_u", C.c_void_p), ("ln_v", C.c_void_p), ("ln_uv_batch_stride", C.c_int64),
-                ("ln_dim", C.c_int32), ("ln_eps", C.c_float), ("res_epilogue", C.c_int32), ("epi_warps", C.c_int32),
-                ("reverse_tiles", C.c_int32)]
+                ("ln_dim", C.c_int32), ("ln_eps", C.c_float), ("reverse_tiles", C.c_int32)]
 
 
 class GemmTail(C.Structure):
@@ -49,14 +48,6 @@ class LnPrepareArgs(C.Structure):
     _fields_ = [("x", C.c_void_p), ("a_out", C.c_void_p), ("stats_out", C.c_void_p), ("scale", C.c_void_p),
                 ("mod_batch_stride", C.c_int64), ("rows_per_batch", C.c_int32), ("M", C.c_int32), ("C", C.c_int32),
                 ("ldx", C.c_int32)]
-
-
-class MlpArgs(C.Structure):
-    _fields_ = [("x", C.c_void_p), ("w1", C.c_void_p), ("b1", C.c_void_p), ("w2", C.c_void_p), ("b2", C.c_void_p), ("x32", C.c_void_p),
-                ("gate", C.c_void_p), ("gate_batch_stride", C.c_int64), ("hidden_ws", C.c_void_p), ("hidden_ws_bytes", C.c_int64),
-                ("flags_ws", C.c_void_p), ("flags_ws_bytes", C.c_int64), ("rows_per_batch", C.c_int32), ("M", C.c_int32),
-                ("K1", C.c_int32), ("N1", C.c_int32), ("N2", C.c_int32), ("ldx", C.c_int32), ("ldw1", C.c_int32), ("ldw2", C.c_int32),
-                ("ldo", C.c_int32), ("group", C.c_int32), ("ring", C.c_int32), ("max_ctas", C.c_int32), ("lag", C.c_int32), ("k_splits", C.c_int32)]
 
 
 class AdamWArgs(C.Structure):
@@ -106,8 +97,8 @@ class AttnArgs(C.Structure):
                 ("k_sn", C.c_int64), ("k_sh", C.c_int64), ("v_sn", C.c_int64), ("v_sh", C.c_int64),
                 ("kv_rows", C.c_int64),
                 ("B", C.c_int32), ("H", C.c_int32), ("Nq", C.c_int32), ("Nk", C.c_int32),
-                ("ldo", C.c_int32), ("scale", C.c_float), ("debug_trace", C.c_void_p), ("lse", C.c_void_p),
-                ("reverse_batch", C.c_int32), ("variant", C.c_int32), ("p_precision", C.c_int32), ("reserved0", C.c_int32)]
+                ("ldo", C.c_int32), ("scale", C.c_float), ("lse", C.c_void_p),
+                ("reverse_batch", C.c_int32), ("p_precision", C.c_int32)]
 
 
 class T5AttnArgs(C.Structure):
@@ -245,8 +236,8 @@ EXPORTS = ("pxa_transpose_bf16", "pxa_gelu_tanh_bf16", "pxa_gate_residual_fwd", 
            "pxa_ln_modulate_bwd", "pxa_colsum_bf16", "pxa_attn_delta_d72", "pxa_flash_attn_d72_bwd_bf16", "pxa_kv_compress_conv2_ln_bwd",
            "pxa_version", "pxa_last_error", "pxa_launch_count", "pxa_gemm_bf16", "pxa_ln_modulate",
            "pxa_flash_attn_d72_bf16", "pxa_kv_compress_conv2_ln", "pxa_conv3x3_nhwc_bf16", "pxa_dpm_solver_pp_step",
-           "pxa_ln_prepare", "pxa_layernorm_affine_bf16", "pxa_groupnorm_silu_nhwc_bf16", "pxa_adamw_flat", "pxa_mlp_fused_bf16",
-           "pxa_rmsnorm_bf16", "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step", "pxa_iddpm_step",
+           "pxa_ln_prepare", "pxa_layernorm_affine_bf16", "pxa_groupnorm_silu_nhwc_bf16", "pxa_adamw_flat", "pxa_rmsnorm_bf16",
+           "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step", "pxa_iddpm_step",
            "pxa_grad_clip_flat", "pxa_came_workspace_bytes", "pxa_came_flat",
            "pxa_lcm_step", "pxa_lcm_teacher_target", "pxa_lcm_consistency_loss", "pxa_ema_flat",
            "pxa_dmd_loss", "pxa_gemm_lora_bf16", "pxa_vae_out_u8")
@@ -268,7 +259,7 @@ def load() -> C.CDLL:
                              ("pxa_flash_attn_d72_bf16", AttnArgs), ("pxa_kv_compress_conv2_ln", KvCompressArgs),
                              ("pxa_conv3x3_nhwc_bf16", Conv3x3Args), ("pxa_dpm_solver_pp_step", DpmStepArgs),
                              ("pxa_ln_prepare", LnPrepareArgs), ("pxa_adamw_flat", AdamWArgs),
-                             ("pxa_mlp_fused_bf16", MlpArgs), ("pxa_t5_attn_d64_bf16", T5AttnArgs),
+                             ("pxa_t5_attn_d64_bf16", T5AttnArgs),
                              ("pxa_sa_solver_step", SaStepArgs), ("pxa_iddpm_step", IddpmStepArgs),
                              ("pxa_grad_clip_flat", GradClipArgs),
                              ("pxa_came_flat", CameArgs), ("pxa_lcm_step", LcmStepArgs),
@@ -337,12 +328,10 @@ def _dt(dtype: torch.dtype) -> int:
 def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: torch.Tensor, *,
          epilogue: int = EPI_BIAS, residual: Optional[torch.Tensor] = None, gate: Optional[torch.Tensor] = None,
          gate_batch_stride: int = 0, rows_per_batch: int = 0, out_aux: Optional[torch.Tensor] = None,
-         block_n: int = 0, max_ctas: int = 0, cta_pair: int = 0, debug_trace: Optional[torch.Tensor] = None,
-         aux_is_branch: bool = False, aux_scale: Optional[torch.Tensor] = None, aux_scale_batch_stride: int = 0,
+         block_n: int = 0, max_ctas: int = 0, aux_is_branch: bool = False, aux_scale: Optional[torch.Tensor] = None, aux_scale_batch_stride: int = 0,
          row_stats_out: Optional[torch.Tensor] = None, ln_stats: Optional[torch.Tensor] = None,
          ln_u: Optional[torch.Tensor] = None, ln_v: Optional[torch.Tensor] = None, ln_uv_batch_stride: int = 0,
-         ln_dim: int = 0, ln_eps: float = 1e-6, res_epilogue: int = 0, epi_warps: int = 0,
-         reverse_tiles: bool = False, tail_a: Optional[torch.Tensor] = None,
+         ln_dim: int = 0, ln_eps: float = 1e-6, reverse_tiles: bool = False, tail_a: Optional[torch.Tensor] = None,
          tail_w: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out = epilogue(a @ w.T + bias). a (M,K) bf16, w (N,K) bf16 (nn.Linear layout), both K-contiguous.
 
@@ -373,11 +362,10 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: to
                     residual=_ptr(residual), gate=_ptr(gate), gate_batch_stride=gate_batch_stride,
                     rows_per_batch=rows_per_batch or M, M=M, N=N, K=K, lda=a.stride(0), ldw=w.stride(0),
                     ldo=out.stride(0), epilogue=epilogue, out_dtype=_dt(out.dtype), block_n=block_n, max_ctas=max_ctas,
-                    cta_pair=cta_pair, debug_trace=_ptr(debug_trace), operands_mn_major=0, k_splits=0,
+                    operands_mn_major=0, k_splits=0,
                     aux_is_branch=int(aux_is_branch), aux_scale=_ptr(aux_scale), aux_scale_batch_stride=aux_scale_batch_stride,
                     row_stats_out=_ptr(row_stats_out), ln_stats=_ptr(ln_stats), ln_u=_ptr(ln_u), ln_v=_ptr(ln_v),
-                    ln_uv_batch_stride=ln_uv_batch_stride, ln_dim=ln_dim, ln_eps=ln_eps, res_epilogue=res_epilogue,
-                    epi_warps=epi_warps, reverse_tiles=int(reverse_tiles))
+                    ln_uv_batch_stride=ln_uv_batch_stride, ln_dim=ln_dim, ln_eps=ln_eps, reverse_tiles=int(reverse_tiles))
     if tail_a is None and tail_w is None:
         _check(load().pxa_gemm_bf16(C.byref(args), _stream()), "pxa_gemm_bf16")
         return out
@@ -417,9 +405,6 @@ def ln_modulate(x: torch.Tensor, shift: torch.Tensor, scale: torch.Tensor, out: 
                      reverse_rows=int(reverse_rows), max_ctas=max_ctas)
     _check(load().pxa_ln_modulate(C.byref(args), _stream()), "pxa_ln_modulate")
     return out
-
-
-_ATTN_VARIANT = int(os.environ.get("PXA_ATTN_VARIANT", "0"))      # A/B switch for the attention forward (0 = library default)
 
 
 def layernorm_affine_(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
@@ -466,8 +451,7 @@ def t5_attn(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor
 def flash_attn(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, *, B: int, H: int, Nq: int,
                Nk: int, kv_rows: int, kv_len: Optional[torch.Tensor] = None, kv_off: Optional[torch.Tensor] = None,
                q_strides=None, k_strides=None, v_strides=None, scale: Optional[float] = None,
-               debug_trace: Optional[torch.Tensor] = None, lse: Optional[torch.Tensor] = None,
-               variant: int = 0, reverse_batch: bool = False, fp32_p: bool = False) -> torch.Tensor:
+               lse: Optional[torch.Tensor] = None, reverse_batch: bool = False, fp32_p: bool = False) -> torch.Tensor:
     """Head-dim-72 attention. q/k/v are bf16 *views*; strides are (row, head) in elements, e.g. slices of the
     (rows, 3, H, 72) qkv GEMM output. out is (B*Nq, H*72) bf16.  fp32_p: `fp32_attention` grade P V (P as bf16 hi + lo)."""
     assert q.dtype == k.dtype == v.dtype == out.dtype == torch.bfloat16
@@ -478,8 +462,7 @@ def flash_attn(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Ten
                     q_sn=q_strides[0], q_sh=q_strides[1], k_sn=k_strides[0], k_sh=k_strides[1],
                     v_sn=v_strides[0], v_sh=v_strides[1], kv_rows=kv_rows, B=B, H=H, Nq=Nq, Nk=Nk,
                     ldo=out.stride(0), scale=scale if scale is not None else 72 ** -0.5,
-                    debug_trace=_ptr(debug_trace), lse=_ptr(lse), variant=variant or _ATTN_VARIANT,
-                    reverse_batch=int(reverse_batch), p_precision=int(bool(fp32_p)), reserved0=0)
+                    lse=_ptr(lse), reverse_batch=int(reverse_batch), p_precision=int(bool(fp32_p)))
     if lse is not None:
         assert lse.dtype == torch.float32 and lse.is_contiguous() and lse.numel() == B * H * Nq
     _check(load().pxa_flash_attn_d72_bf16(C.byref(args), _stream()), "pxa_flash_attn_d72_bf16")
@@ -531,43 +514,6 @@ def vae_out_u8(x: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor, out_
                       x_sh=x.stride(1), x_sw=x.stride(2), B=B, H=H, W=W, Cin=Cin)
     _check(load().pxa_vae_out_u8(C.byref(args), _stream()), "pxa_vae_out_u8")
     return out_u8
-
-
-def _env_int(name: str, default: int) -> int:
-    return int(os.environ.get(name, default))
-
-
-# fc2 trails fc1 by LAG groups of GROUP 256-row panels; the ring holds RING = LAG + 2 groups (mlp_sm90.cu)
-MLP_GROUP, MLP_LAG = _env_int("PXA_MLP_GROUP", 4), _env_int("PXA_MLP_LAG", 1)
-MLP_RING = _env_int("PXA_MLP_RING", MLP_LAG + 2)
-
-
-def mlp_fused_workspace(M: int, n_hidden: int, device, group: int = MLP_GROUP, ring: int = MLP_RING):
-    """(hidden ring, flag array) for `mlp_fused` at M rows."""
-    panels = (M + 255) // 256
-    hidden = torch.empty(ring * group * 256 * n_hidden, dtype=torch.bfloat16, device=device)
-    flags = torch.empty(2 * panels + (panels + group - 1) // group + 4, dtype=torch.int32, device=device)
-    return hidden, flags
-
-
-def mlp_fused(x: torch.Tensor, w1: torch.Tensor, b1: Optional[torch.Tensor], w2: torch.Tensor, b2: Optional[torch.Tensor],
-              x32: torch.Tensor, *, gate: Optional[torch.Tensor] = None, gate_batch_stride: int = 0, rows_per_batch: int = 0,
-              hidden_ws: torch.Tensor, flags_ws: torch.Tensor, group: int = MLP_GROUP, ring: int = MLP_RING, lag: int = MLP_LAG,
-              max_ctas: int = 0, k_splits: int = 0) -> torch.Tensor:
-    """x32 += gate[b] * (gelu_tanh(x @ w1.T + b1) @ w2.T + b2) in ONE persistent kernel (include/pixart_sm100.h, PxaMlpArgs)."""
-    assert x.dtype == w1.dtype == w2.dtype == torch.bfloat16 and x32.dtype == torch.float32 and x.is_cuda
-    assert x.dim() == 2 and x.stride(1) == 1 and w1.stride(1) == 1 and w2.stride(1) == 1 and x32.stride(1) == 1
-    M, K1 = x.shape
-    N1, N2 = w1.shape[0], w2.shape[0]
-    assert w1.shape[1] == K1 and w2.shape[1] == N1 and x32.shape == (M, N2)
-    assert hidden_ws.dtype == torch.bfloat16 and hidden_ws.is_contiguous() and flags_ws.dtype == torch.int32 and flags_ws.is_contiguous()
-    args = MlpArgs(x=_ptr(x), w1=_ptr(w1), b1=_ptr(b1), w2=_ptr(w2), b2=_ptr(b2), x32=_ptr(x32), gate=_ptr(gate),
-                   gate_batch_stride=gate_batch_stride, hidden_ws=_ptr(hidden_ws), hidden_ws_bytes=hidden_ws.numel() * 2,
-                   flags_ws=_ptr(flags_ws), flags_ws_bytes=flags_ws.numel() * 4, rows_per_batch=rows_per_batch or M, M=M, K1=K1,
-                   N1=N1, N2=N2, ldx=x.stride(0), ldw1=w1.stride(0), ldw2=w2.stride(0), ldo=x32.stride(0), group=group, ring=ring,
-                   max_ctas=max_ctas, lag=lag, k_splits=k_splits)
-    _check(load().pxa_mlp_fused_bf16(C.byref(args), _stream()), "pxa_mlp_fused_bf16")
-    return x32
 
 
 def adamw_flat(param: torch.Tensor, grad: torch.Tensor, exp_avg: torch.Tensor, exp_avg_sq: torch.Tensor, *, step: int, lr: float,
@@ -952,7 +898,7 @@ def gemm_wgrad(a_t: torch.Tensor, w_t: torch.Tensor, out: torch.Tensor, *, block
     args = GemmArgs(a=_ptr(a_t), w=_ptr(w_t), bias=None, out=_ptr(out), out_aux_bf16=None, residual=_ptr(out), gate=None,
                     gate_batch_stride=0, rows_per_batch=M, M=M, N=N, K=K, lda=a_t.stride(0), ldw=w_t.stride(0),
                     ldo=out.stride(0), epilogue=EPI_BIAS_RESIDUAL, out_dtype=DTYPE_F32, block_n=block_n, max_ctas=max_ctas,
-                    cta_pair=1, debug_trace=None, operands_mn_major=1, k_splits=k_splits, aux_is_branch=0)
+                    operands_mn_major=1, k_splits=k_splits, aux_is_branch=0)
     _check(load().pxa_gemm_bf16(C.byref(args), _stream()), "pxa_gemm_bf16 (wgrad)")
     return out
 

@@ -253,9 +253,6 @@ class _Workspace:
         return t
 
 
-_MLP_FUSED = os.environ.get("PXA_MLP_FUSED", "0") == "1"   # Mlp branch through pxa_mlp_fused_bf16 (mlp_sm90.cu)
-_L2_CHAIN = os.environ.get("PXA_L2_CHAIN", "1") != "0"      # consumer kernels start on the rows their producer wrote last
-
 _LN_FUSE_MIN_ROWS = 128      # a 128-row GEMM tile may span at most two samples (include/pixart_sm100.h)
 
 
@@ -263,33 +260,6 @@ def _ln_ctx(u: torch.Tensor, v: torch.Tensor, one_plus: torch.Tensor, i: int, st
     """`ln` argument of PixArtMSBlock.run_kernels for block i of a chain (see _LnFusion.prepare)."""
     return {"stats": stats, "u": u[i], "v": v[i], "uv_stride": u.stride(1), "one_plus": one_plus[i], "prepare": i == 0,
             "next_one_plus": one_plus[i + 1] if i + 1 < one_plus.shape[0] else None}
-
-
-class _KvBatch:
-    """All `cross_attn.kv_linear` layers of the model as ONE GEMM per forward (PixArt_blocks.py:48: `self.kv_linear(cond)` with the
-    same `cond` in every block).  28 GEMMs with M = B x text tokens (<= 2400 rows: waves of half-empty tiles)
-    become one with N = depth x 2C.  Owns the row-stacked weight / bias copies, rebuilt when a weight changes."""
-
-    def __init__(self, blocks):
-        self.blocks = list(blocks)
-        self.key = None
-        self.w = self.b = None
-
-    def project(self, cond: torch.Tensor, ws: "_Workspace") -> torch.Tensor:
-        mods = [blk.cross_attn.kv_linear for blk in self.blocks]
-        key = tuple((m.weight._version, m.weight.data_ptr(), m.bias._version, m.bias.data_ptr()) for m in mods)
-        if key != self.key:
-            self.w = torch.cat([m.weight.detach() for m in mods], dim=0).contiguous()          # (depth * 2C, C)
-            self.b = torch.cat([m.bias.detach() for m in mods], dim=0).contiguous()
-            self.key = key
-        out = ws.get("kv_all", (cond.shape[0], self.w.shape[0]), cond.dtype, cond.device)
-        lib.gemm(cond, self.w, self.b, out)
-        return out
-
-
-# Opt-in (PXA_KV_BATCH=1): the FLOPs are the same (its effect on the c3 step has not been measured on the H100), and the stacked
-# copy goes stale under in-place weight writes that bypass the version counter (`p.data.copy_()`: EMA / ZeRO-style updates).
-_KV_BATCH = os.environ.get("PXA_KV_BATCH", "0") == "1"
 
 
 class _LnFusion:
@@ -419,16 +389,13 @@ class PixArtMSBlock(nn.Module):
     # -- the fused path ---------------------------------------------------------------------------------------
     def run_kernels(self, x32: torch.Tensor, cond: torch.Tensor, kv_len: Optional[torch.Tensor],
                     kv_off: Optional[torch.Tensor], max_keys: int, mod: torch.Tensor, B: int, N: int,
-                    HW: Tuple[int, int], ws: _Workspace, ln: Optional[dict] = None,
-                    kv_pre: Optional[torch.Tensor] = None) -> torch.Tensor:
+                    HW: Tuple[int, int], ws: _Workspace, ln: Optional[dict] = None) -> torch.Tensor:
         """One block on the kernels, in place on the fp32 residual stream.
 
         x32  (B*N, C) fp32 residual stream (updated in place and returned)
         cond (rows, C) bf16 embedded caption tokens; sample b's keys are rows kv_off[b] .. +kv_len[b]
              (kv_off None -> b*max_keys, kv_len None -> max_keys)
         mod  (B, 6, C) fp32 = scale_shift_table + t0  (shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp)
-        kv_pre  None, or this block's cross-attention keys / values (rows, 2C) bf16 (a strided view is fine) already projected by
-             `_KvBatch` -- the caption tokens are the same for every block, so PixArtMS.forward runs all kv_linear layers as ONE GEMM.
         ln   None: norm + modulate as a stand-alone pass (pxa_ln_modulate) before the QKV / fc1 GEMMs.
              dict (from `_ln_ctx`): the FUSED form -- LayerNorm + t2i_modulate evaluated inside the QKV / fc1 GEMM epilogues
              from the scaled bf16 copy of x and the row statistics that the preceding residual epilogue left behind.
@@ -468,7 +435,7 @@ class PixArtMSBlock(nn.Module):
         # L2 chaining (126 MB): each kernel starts on the rows its producer wrote last -- the QKV GEMM runs front to back, the
         # attention back to front (so attn.proj, front to back again, finds the first samples' outputs still cached)
         lib.flash_attn(q3[:, 0], k_src, v_src, ao, B=B, H=H, Nq=N, Nk=n_keys, kv_rows=B * n_keys,
-                       q_strides=(3 * C, C // H), k_strides=k_str, v_strides=k_str, scale=a.scale, reverse_batch=_L2_CHAIN,
+                       q_strides=(3 * C, C // H), k_strides=k_str, v_strides=k_str, scale=a.scale, reverse_batch=True,
                        fp32_p=bool(getattr(a, "fp32_attention", False)))
         lib.gemm(ao, a.proj.weight, a.proj.bias, x32, epilogue=lib.EPI_BIAS_RESIDUAL, residual=x32, gate=mod[:, 2],
                  gate_batch_stride=ms, rows_per_batch=N, out_aux=xb)
@@ -476,11 +443,8 @@ class PixArtMSBlock(nn.Module):
         # (2) x += proj(cross_attn(x, cond))            (no norm, no gate)                       PixArtMS.py:76
         qx = ws.get("q_cross", (M, C), bf, dev)
         lib.gemm(xb, ca.q_linear.weight, ca.q_linear.bias, qx)
-        if kv_pre is None:
-            kv = ws.get("kv_cross", (cond.shape[0], 2 * C), bf, dev)
-            lib.gemm(cond, ca.kv_linear.weight, ca.kv_linear.bias, kv)
-        else:
-            kv = kv_pre
+        kv = ws.get("kv_cross", (cond.shape[0], 2 * C), bf, dev)
+        lib.gemm(cond, ca.kv_linear.weight, ca.kv_linear.bias, kv)
         kv4 = kv.view(-1, 2, H, C // H)
         lib.flash_attn(qx, kv4[:, 0], kv4[:, 1], ao, B=B, H=H, Nq=N, Nk=max_keys, kv_rows=cond.shape[0],
                        kv_len=kv_len, kv_off=kv_off, q_strides=(C, C // H), k_strides=(kv.stride(0), C // H),
@@ -492,21 +456,13 @@ class PixArtMSBlock(nn.Module):
             lib.gemm(ao, ca.proj.weight, ca.proj.bias, x32, epilogue=lib.EPI_BIAS_RESIDUAL, residual=x32)
 
         # (3) x += gate_mlp * fc2(gelu_tanh(fc1(LN(x) * (1 + scale_mlp) + shift_mlp)))           PixArtMS.py:77
-        if self._mlp_one_kernel(N, M) and not fused:
-            # the whole Mlp branch per group of row panels, hidden activations resident in L2 (mlp_sm90.cu)
-            lib.ln_modulate(x32, mod[:, 3], mod[:, 4], xn, mod_batch_stride=ms, rows_per_batch=N, reverse_rows=_L2_CHAIN)
-            hws = ws.get("mlp_ring", (lib.MLP_RING * lib.MLP_GROUP * 256 * mlp.fc1.out_features,), bf, dev)
-            fws = ws.get("mlp_flags", (3 * ((M + 255) // 256) + 8,), torch.int32, dev)
-            lib.mlp_fused(xn, mlp.fc1.weight, mlp.fc1.bias, mlp.fc2.weight, mlp.fc2.bias, x32, gate=mod[:, 5], gate_batch_stride=ms,
-                          rows_per_batch=N, hidden_ws=hws, flags_ws=fws)
-            return x32
         hid = ws.get("mlp_hidden", (M, mlp.fc1.out_features), bf, dev)
         if fused:
             lib.gemm(xn, mlp.fc1.weight, None, hid, epilogue=lib.EPI_LN_BIAS_GELU, rows_per_batch=N, ln_u=u[:, n1:], ln_v=v[:, n1:],
                      **lnkw)
         else:
             # back to front: the rows of x the (front-to-back) cross-attention projection wrote last are still in L2
-            lib.ln_modulate(x32, mod[:, 3], mod[:, 4], xn, mod_batch_stride=ms, rows_per_batch=N, reverse_rows=_L2_CHAIN)
+            lib.ln_modulate(x32, mod[:, 3], mod[:, 4], xn, mod_batch_stride=ms, rows_per_batch=N, reverse_rows=True)
             lib.gemm(xn, mlp.fc1.weight, mlp.fc1.bias, hid, epilogue=lib.EPI_BIAS_GELU)
         nxt = ln.get("next_one_plus") if fused else None
         if nxt is not None:                         # ... and here A / statistics for the NEXT block's norm1
@@ -515,12 +471,8 @@ class PixArtMSBlock(nn.Module):
                      row_stats_out=stats)
         else:       # back to front: the hidden rows fc1 wrote last (302 MB in all at c3) are the ones still in L2
             lib.gemm(hid, mlp.fc2.weight, mlp.fc2.bias, x32, epilogue=lib.EPI_BIAS_RESIDUAL, residual=x32, gate=mod[:, 5],
-                     gate_batch_stride=ms, rows_per_batch=N, reverse_tiles=_L2_CHAIN)
+                     gate_batch_stride=ms, rows_per_batch=N, reverse_tiles=True)
         return x32
-
-    def _mlp_one_kernel(self, N: int, M: int) -> bool:
-        """Use pxa_mlp_fused_bf16 for the Mlp branch?  (PXA_MLP_FUSED=1; shapes the kernel is built for)"""
-        return (_MLP_FUSED and N >= 128 and self.mlp.fc1.out_features % 256 == 0 and self.mlp.fc2.out_features % 192 == 0)
 
     def _compress_kv(self, qkv, B, N, HW, ws):
         """K / V token compression (PixArt_blocks.py:97-121). 'conv' sr=2 runs the fused conv+LN kernel; the
@@ -644,7 +596,6 @@ class PixArtMS(nn.Module):
         # norm passes they remove; which side wins has not been measured on the H100.  PXA_FUSE_LN=1 turns it on.
         self.fuse_ln_modulate = os.environ.get("PXA_FUSE_LN", "0") == "1"
         self.__dict__["_ln_fusion"] = None
-        self.__dict__["_kv_batch"] = None
         self._ws = _Workspace()
         self.initialize()
 
@@ -734,15 +685,9 @@ class PixArtMS(nn.Module):
                 self.__dict__["_ln_fusion"] = _LnFusion(self.blocks)
             u, v, one_plus = self._ln_fusion.prepare(t0.view(B, 6, C), mod_all, self._ws)
             stats = self._ws.get("ln_stats", (B * N, lib.LN_STAT_PARTS, 2), torch.float32, dev)
-        kv_all = None
-        if _KV_BATCH and len(self.blocks) > 1:
-            if self._kv_batch is None:
-                self.__dict__["_kv_batch"] = _KvBatch(self.blocks)
-            kv_all = self._kv_batch.project(cond, self._ws)
         for i, blk in enumerate(self.blocks):
             blk.run_kernels(x32, cond, kv_len, None, max_keys, mod_all[i], B, N, (self.h, self.w), self._ws,
-                            _ln_ctx(u, v, one_plus, i, stats) if fused else None,
-                            None if kv_all is None else kv_all[:, i * 2 * C:(i + 1) * 2 * C])
+                            _ln_ctx(u, v, one_plus, i, stats) if fused else None)
 
         fl = self.final_layer                                                                  # uses t, not t0 (:208)
         fmod = (fl.scale_shift_table.float()[None] + t[:, None]).contiguous()                  # (B, 2, C): shift, scale

@@ -39,11 +39,11 @@ def _denoiser_params(model: Callable) -> list:
 
 def _denoiser_key(model: Callable, params: list, model_kwargs: Optional[dict]) -> tuple:
     """The denoiser's part of a captured sampling loop's cache key.  `model_kwargs` tensors are captured by address, and so
-    are the denoiser's parameters: the forward keeps derived copies (stacked kv_linear weights) a replay cannot refresh."""
+    are the denoiser's parameters: the fused-LN forward keeps tables derived from them that a replay cannot refresh."""
     kw_id = tuple(sorted((k, (v.data_ptr(), tuple(v.shape)) if isinstance(v, torch.Tensor) else repr(v))
                          for k, v in (model_kwargs or {}).items()))
     owner = getattr(model, "__self__", model)
-    derived = getattr(owner, "_kv_batch", None) is not None or getattr(owner, "_ln_fusion", None) is not None
+    derived = getattr(owner, "_ln_fusion", None) is not None
     wkey = (sum(p._version for p in params), params[0].data_ptr()) if (params and derived) else None
     return kw_id, wkey
 

@@ -1,8 +1,8 @@
 """Float64 references and element-wise error bounds for the wgmma GEMM family (gemm_sm100.cu): every epilogue of
-pxa_gemm_bf16, the LoRA K-tail of pxa_gemm_lora_bf16, the split-K weight gradient, the implicit-GEMM 3x3 convolution, the
-fused LayerNorm chain (pxa_ln_prepare, aux_scale / row_stats_out, EPI_LN_*) and pxa_mlp_fused_bf16.  Shared by
-test_gemm_numerics_cpu.py, which checks the bounds against float32 emulations of the kernels, and test_gemm_numerics_gpu.py,
-which checks the kernels against them.
+pxa_gemm_bf16, the LoRA K-tail of pxa_gemm_lora_bf16, the split-K weight gradient, the implicit-GEMM 3x3 convolution and the
+fused LayerNorm chain (pxa_ln_prepare, aux_scale / row_stats_out, EPI_LN_*).  Shared by test_gemm_numerics_cpu.py, which
+checks the bounds against float32 emulations of the kernels, and test_gemm_numerics_gpu.py, which checks the kernels against
+them.
 
 Every output o is checked as
     |o_kernel - o_ref| <= c ulp(|o_ref| + slack) + slack,
@@ -50,8 +50,6 @@ Epilogues (y = acc + bias, formed in fp32: slack_y = slack_acc + u |y|):
         slack = rstd slack_acc + rel(rstd) rstd |acc| + e(c) |u_b| + u |c u_b + v_b| + u |x|.
     The rstd |acc| and e(c) |u| terms grow like |mu| rstd: this is the fused form's trade-off (see
     test_fused_ln_epilogue_error_grows_with_offset_as_designed for its effect against an unfused LayerNorm).
-  - pxa_mlp_fused_bf16: the fp32-residual bound of fc2 plus |gate| sum_j |w2_nj| (1 ulp(h_j) + (|gelu'| + 0.8 s) s_j + 2^-40),
-    s_j the fc1 slack: the bf16 hidden layer is internal, so the reference is fc2 of the exact gelu(fc1).
 
 Bias: `Tally` also reports mean(sign(ref) (got - ref) / bound) over the elements with |ref| > `tiny`.  Round to nearest
 leaves it near 0; a store that rounds toward zero pulls every element's error towards -sign(ref) and moves the mean by about

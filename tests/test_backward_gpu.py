@@ -148,24 +148,24 @@ def test_gemm_residual_epilogue_keeps_the_branch_output(K):
     assert po.rel_err(y.float(), branch) < 4e-3
 
 
-@pytest.mark.parametrize("M,N,K,pair", [(2048, 4608, 1152, 0), (512, 256, 128, 1), (1000, 4608, 1152, 2)])
-def test_gemm_gelu_epilogue_keeps_the_pre_activation(M, N, K, pair):
+@pytest.mark.parametrize("M,N,K", [(2048, 4608, 1152), (512, 256, 128), (1000, 4608, 1152)])
+def test_gemm_gelu_epilogue_keeps_the_pre_activation(M, N, K):
     a, w, bias = _randn(M, K, seed=70), _randn(N, K, seed=71, scale=K ** -0.5), _randn(N, seed=72, scale=0.1)
     h = torch.full((M, N), float("nan"), dtype=torch.bfloat16, device=DEV)
     pre = torch.full((M, N), float("nan"), dtype=torch.bfloat16, device=DEV)
-    lib.gemm(a, w, bias, h, epilogue=lib.EPI_BIAS_GELU_AUX, out_aux=pre, cta_pair=pair)
+    lib.gemm(a, w, bias, h, epilogue=lib.EPI_BIAS_GELU_AUX, out_aux=pre)
     want = F.linear(a.float(), w.float(), bias.float())
     assert po.rel_err(pre.float(), want) < 4e-3
     assert po.rel_err(h.float(), F.gelu(want, approximate="tanh")) < 4e-3
 
 
-@pytest.mark.parametrize("M,N,K,pair", [(2048, 4608, 1152, 0), (512, 256, 128, 1), (1000, 4608, 1152, 2)])
-def test_gemm_dgelu_epilogue(M, N, K, pair):
+@pytest.mark.parametrize("M,N,K", [(2048, 4608, 1152), (512, 256, 128), (1000, 4608, 1152)])
+def test_gemm_dgelu_epilogue(M, N, K):
     """dgrad GEMM of the MLP's second layer with gelu'(pre) applied in the epilogue: out = (dy W) * gelu'(pre)."""
     dy, wt = _randn(M, K, seed=73), _randn(N, K, seed=74, scale=K ** -0.5)          # wt = W^T rows (N = hidden)
     pre = _randn(M, N, seed=75, scale=1.5)
     out = torch.full((M, N), float("nan"), dtype=torch.bfloat16, device=DEV)
-    lib.gemm(dy, wt, None, out, epilogue=lib.EPI_MUL_DGELU, residual=pre, cta_pair=pair)
+    lib.gemm(dy, wt, None, out, epilogue=lib.EPI_MUL_DGELU, residual=pre)
     x = pre.float().requires_grad_(True)
     F.gelu(x, approximate="tanh").backward(F.linear(dy.float(), wt.float()))
     assert po.rel_err(out.float(), x.grad) < 5e-3

@@ -1,6 +1,6 @@
 """The wgmma GEMM family (-m gpu) element by element against float64, on real (non-integer) data at the model's shapes
 (XL/2: C = 1152, MLP 4608, 2048 image rows = B = 2 at 512 px, 600 caption rows, unless noted): every epilogue of pxa_gemm_bf16, the LoRA down-projection
-and K-tail, the split-K weight gradient, the 3x3 convolution, the fused LayerNorm chain and pxa_mlp_fused_bf16.  The bounds
+and K-tail, the split-K weight gradient, the 3x3 convolution and the fused LayerNorm chain.  The bounds
 and their derivation are in gemm_bounds.py; test_gemm_numerics_cpu.py shows they are attainable and reject the defects they
 are meant to catch.
 
@@ -415,33 +415,3 @@ def test_ln_epilogue_formula(ratio, gelu):
         gb.Tally(name, c=1.0, tiny=gb.GELU_TINY).add(got, *gb.gelu_out(xr, sx)).check()
     else:
         gb.Tally(name).add(got, xr, sx).check()
-
-
-# ------------------------------------------------------------------------------------------------- fused MLP
-@pytest.mark.parametrize("M,rpb,max_ctas,group,ring", [(2304, 1152, 0, 4, 3), (1000, 500, 0, 2, 2), (4096, 1024, 6, 2, 2),
-                                                       (5120, 1024, 20, 1, 2)])
-def test_mlp_fused(M, rpb, max_ctas, group, ring):
-    """x32 += gate (gelu(x W1^T + b1) W2^T + b2): the fp32-residual bound of fc2 plus the hidden layer's slack carried
-    through |W2| (gemm_bounds.py), against fc2 of the exact float64 GELU."""
-    xn = rnd(M, C, seed=160)
-    w1, b1 = rnd(HID, C, seed=161, scale=3 * C ** -0.5), rnd(HID, seed=162, scale=0.1)
-    w2, b2 = rnd(C, HID, seed=163, scale=HID ** -0.5), rnd(C, seed=164, scale=0.1)
-    x32 = rnd(M, C, seed=165, dtype=F32)
-    g, gd = gates(M, C, rpb, seed=166)
-    acc1, s1 = acc_of(xn, w1)
-    y1, sy1 = gb.bias_out(acc1, s1, d(b1))
-    h, sh = gb.gelu_out(y1, sy1)
-    sh = sh + gb.bf16_ulp(h.abs() + sh)                          # the bf16 hidden layer: 1 ulp, the GELU's contract
-    w2d = d(w2)
-    acc2 = h @ w2d.T
-    s2 = gb.accumulate(h.to(BF).double(), w2d)[1] + sh @ w2d.abs().T
-    y2, sy2 = gb.bias_out(acc2, s2, d(b2))
-    o, so = gb.residual_out(y2, sy2, gd, d(x32))
-    out, buf = gb.sentinel_out(M, C, F32, DEV, fill=x32)
-    hws, fws = lib.mlp_fused_workspace(M, HID, DEV, group=group, ring=ring)
-    hws.fill_(float("nan"))
-    lib.mlp_fused(gb.nan_padded(xn), gb.nan_padded(w1), b1, gb.nan_padded(w2), b2, out, gate=g, gate_batch_stride=2 * C,
-                  rows_per_batch=rpb, hidden_ws=hws, flags_ws=fws, group=group, ring=ring, max_ctas=max_ctas)
-    torch.cuda.synchronize()
-    gb.assert_guard(buf, M, C, "x32")
-    gb.Tally(f"mlp_fused M {M} group {group} ring {ring} max_ctas {max_ctas}", fp32=True).add(out.double(), o, so).check()

@@ -97,22 +97,25 @@ def test_library_exports_every_symbol_the_header_declares():
     assert dll.pxa_version() == 100
 
 
-def test_ctypes_structs_match_header_sizes():
-    """Field-by-field size check of the POD argument structs against a compile of the header with gcc."""
+def test_ctypes_struct_fields_match_the_header():
+    """Every ctypes argument struct X of lib against the header's PxaX compiled with gcc: the size of the struct and the offset
+    of each field (a field dropped on one side only can leave the size unchanged and still shift the fields after it)."""
     import subprocess, tempfile
-    src = '#include <stdio.h>\n#include "pixart_sm100.h"\nint main(){printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(PxaGemmArgs),' \
-          ' sizeof(PxaLnModArgs), sizeof(PxaAttnArgs), sizeof(PxaKvCompressArgs), sizeof(PxaConv3x3Args),' \
-          ' sizeof(PxaDpmStepArgs), sizeof(PxaGateResidualArgs), sizeof(PxaLnModBwdArgs), sizeof(PxaAttnBwdArgs),' \
-          ' sizeof(PxaKvCompressBwdArgs), sizeof(PxaLnPrepareArgs), sizeof(PxaAdamWArgs), sizeof(PxaMlpArgs), sizeof(PxaT5AttnArgs));return 0;}\n'
+    structs = {n: s for n, s in vars(lib).items()
+               if isinstance(s, type) and issubclass(s, ctypes.Structure) and s.__module__ == lib.__name__}
+    want, probes = {}, []
+    for name, s in structs.items():
+        want[name] = ctypes.sizeof(s)
+        probes.append(f'printf("{name} %zu\\n", sizeof(Pxa{name}));')
+        for f in s._fields_:
+            want[f"{name}.{f[0]}"] = getattr(s, f[0]).offset
+            probes.append(f'printf("{name}.{f[0]} %zu\\n", offsetof(Pxa{name}, {f[0]}));')
+    src = '#include <stddef.h>\n#include <stdio.h>\n#include "pixart_sm100.h"\nint main(void) {\n' + "\n".join(probes) + "\nreturn 0;\n}\n"
     with tempfile.TemporaryDirectory() as d:
         open(os.path.join(d, "s.c"), "w").write(src)
         subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), os.path.join(d, "s.c"), "-o", os.path.join(d, "s")])
-        sizes = [int(v) for v in subprocess.check_output([os.path.join(d, "s")]).split()]
-    assert sizes == [ctypes.sizeof(lib.GemmArgs), ctypes.sizeof(lib.LnModArgs), ctypes.sizeof(lib.AttnArgs),
-                     ctypes.sizeof(lib.KvCompressArgs), ctypes.sizeof(lib.Conv3x3Args), ctypes.sizeof(lib.DpmStepArgs),
-                     ctypes.sizeof(lib.GateResidualArgs), ctypes.sizeof(lib.LnModBwdArgs), ctypes.sizeof(lib.AttnBwdArgs),
-                     ctypes.sizeof(lib.KvCompressBwdArgs), ctypes.sizeof(lib.LnPrepareArgs), ctypes.sizeof(lib.AdamWArgs), ctypes.sizeof(lib.MlpArgs),
-                     ctypes.sizeof(lib.T5AttnArgs)]
+        got = {k: int(v) for k, v in (line.split() for line in subprocess.check_output([os.path.join(d, "s")], text=True).splitlines())}
+    assert got == want
 
 
 def test_integration_md_ctypes_stub_matches_the_header_struct():

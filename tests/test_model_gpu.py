@@ -240,36 +240,6 @@ def test_cuda_graph_replay_equals_eager():
     assert not torch.equal(outs[0], outs[1])
 
 
-def test_batched_kv_projection_equals_per_block_and_follows_weight_updates():
-    """All cross_attn.kv_linear layers as ONE GEMM per forward (model._KvBatch) against the per-block GEMMs: same K loop per output
-    element, so the forward is bit-identical; an in-place weight update is picked up eagerly and by GraphedForward (which drops
-    its captured graphs when a parameter version changes)."""
-    from pixart_sigma_b200 import model as pm
-    from pixart_sigma_b200.graph import GraphedForward
-    cfg = po.OracleConfig(depth=3, input_size=32, pe_interpolation=0.5)
-    m = _build(cfg, po.synthetic_state_dict(cfg, seed=3))
-    x, t, y, mask = (v.cuda() for v in po.synthetic_inputs(cfg, 2, (32, 32), lens=[300, 33]))
-    was = pm._KV_BATCH
-    try:
-        with torch.no_grad():
-            pm._KV_BATCH = True
-            batched = m(x, t, y, mask=mask).clone()
-            pm._KV_BATCH = False
-            per_block = m(x, t, y, mask=mask).clone()
-            assert torch.equal(batched, per_block)
-            pm._KV_BATCH = True
-            gf = GraphedForward(m, "forward")
-            assert torch.equal(gf(x, t, y.to(torch.bfloat16), mask), batched)
-            m.blocks[1].cross_attn.kv_linear.weight.mul_(1.5)          # in place: same storage, new version
-            changed = m(x, t, y, mask=mask).clone()
-            assert not torch.equal(changed, batched)
-            assert torch.equal(gf(x, t, y.to(torch.bfloat16), mask), changed)
-            pm._KV_BATCH = False
-            assert torch.equal(m(x, t, y, mask=mask), changed)
-    finally:
-        pm._KV_BATCH = was
-
-
 def test_fp16_checkpoint_is_cast_to_bf16_once_and_keeps_fp16_io():
     """scripts/inference.py:161 loads the model as fp16 (`weight_dtype = torch.float16`): the first forward casts the
     parameters to bf16 in place (with a warning), later calls are silent, outputs stay fp16."""
