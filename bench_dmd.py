@@ -45,7 +45,7 @@ def event_shares(dist, b, y, mask, update_gen, update_fake):
     from pixart_sigma_b200 import autograd as ag
     from pixart_sigma_b200 import lib
     from pixart_sigma_b200.dmd import _DmdLoss
-    from pixart_sigma_b200.sampler import _step_input
+    from pixart_sigma_b200.capture import step_input
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(11)]
     for _ in range(2):
         for red in (dist.gen_reducer, dist.fake_reducer):
@@ -60,7 +60,7 @@ def event_shares(dist, b, y, mask, update_gen, update_fake):
         ev[1].record()
         with torch.no_grad():
             latents, scratch = torch.empty_like(init_noise), torch.empty_like(init_noise)
-            lib.lcm_step(_step_input(out_g[:, :4]), init_noise, None, latents, scratch, **dist.gen_scalars)
+            lib.lcm_step(step_input(out_g[:, :4]), init_noise, None, latents, scratch, **dist.gen_scalars)
             noisy = dist.add_noise(latents, noise, t).contiguous()
             uy = dist.uncond_y.to(dtype=y.dtype).expand(b, *dist.uncond_y.shape[1:])
             m2 = torch.cat([dist.uncond_mask.to(mask.dtype).expand(b, -1), mask])
@@ -69,7 +69,7 @@ def event_shares(dist, b, y, mask, update_gen, update_fake):
         ag.refresh_shadows(dist.fake)
         fake_out = dist.fake(noisy, t, y, mask=mask).detach()
         ev[3].record()
-        dm = _DmdLoss.apply(out_g, latents, noisy, t, dist.ac, _step_input(real_out), _step_input(fake_out), partials, weight,
+        dm = _DmdLoss.apply(out_g, latents, noisy, t, dist.ac, step_input(real_out), step_input(fake_out), partials, weight,
                             dist.cfg, dist.gen_scalars["sqrt_alpha"], dist.gen_scalars["sqrt_beta"])
         ev[4].record()
         dm.backward()

@@ -62,7 +62,7 @@ def event_shares(student, red, dist, update, x, y, mask, b):
     gradient accumulators keep the stream they were created on."""
     from pixart_sigma_b200 import autograd as ag
     from pixart_sigma_b200 import lcm, lib
-    from pixart_sigma_b200.sampler import _step_input
+    from pixart_sigma_b200.capture import step_input
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(8)]
     for _ in range(2):
         red.zero_grad()
@@ -79,11 +79,11 @@ def event_shares(student, red, dist, update, x, y, mask, b):
             uncond = dist.uncond.to(dtype=y.dtype).expand(b, 1, *dist.uncond.shape)
             out_t = dist.teacher(torch.cat([x_t, x_t]), torch.cat([start, start]), torch.cat([y, uncond]), mask=torch.cat([mask, mask]))
             x_prev = torch.empty_like(x_t)
-            lib.lcm_teacher_target(_step_input(out_t), x_t, index, dist.table, x_prev, w=dist.w)
+            lib.lcm_teacher_target(step_input(out_t), x_t, index, dist.table, x_prev, w=dist.w)
             ev[2].record()
             out_e = dist.ema(x_prev, t, y, mask=mask)
         ev[3].record()
-        loss = lcm._ConsistencyLoss.apply(out_s, _step_input(out_e), x_t, x_prev, index, dist.table, dist.partials,
+        loss = lcm._ConsistencyLoss.apply(out_s, step_input(out_e), x_t, x_prev, index, dist.table, dist.partials,
                                           dist.loss_type, dist.huber_c)
         ev[4].record()
         loss.backward()

@@ -26,7 +26,7 @@ import torch
 
 from . import lib
 from .lcm import FlatEMA, LCMScheduler, _ConsistencyLoss, _dup, _inference_copy, _upload
-from .sampler import _capture, _denoiser_key, _denoiser_params, _step_input
+from .capture import CapturedLoops, step_input
 
 __all__ = ["ddpm_alphas_cumprod", "ddpm_add_noise", "ema_decay", "dmd_draws", "null_caption", "DMDSampler", "DMDDistiller"]
 
@@ -111,12 +111,11 @@ class DMDSampler:
             raise ValueError(f"timestep must be in [0, {num_train_timesteps})")
         self.model, self.timestep = model_fn, int(timestep)
         self.scalars = _x0_scalars(ddpm_alphas_cumprod(num_train_timesteps), self.timestep)
-        self._params = _denoiser_params(model_fn)
-        self._graphs: Dict[tuple, tuple] = {}
+        self._graphs = CapturedLoops()
 
     def _run(self, x, den, ts, model_kwargs):
         out = self.model(x, ts, **model_kwargs)
-        lib.lcm_step(_step_input(out[:, :4]), x, None, den, x, **self.scalars)
+        lib.lcm_step(step_input(out[:, :4]), x, None, den, x, **self.scalars)
         return den
 
     @torch.no_grad()
@@ -128,29 +127,13 @@ class DMDSampler:
         if x_T.dim() != 4 or x_T.shape[1] != 4 or (x_T.shape[2] * x_T.shape[3]) % 4:
             raise ValueError("x_T must be (n, 4, h, w) latents with h*w a multiple of 4")
         ts = torch.full((x_T.shape[0],), self.timestep, dtype=torch.int64, device=x_T.device)
-        if not cuda_graph:
-            x = x_T.to(torch.float32).contiguous().clone()
+
+        def loop(x0, k, draws):
+            x = x0.to(torch.float32).contiguous().clone()
             return self._run(x, torch.empty_like(x), ts, model_kwargs)
-        # the timestep is baked into the captured launches, model_kwargs tensors and the parameters (through derived weight
-        # copies) into the captured forward: all are part of the key
-        kw_id, wkey = _denoiser_key(self.model, self._params, model_kwargs)
-        key = (tuple(x_T.shape), x_T.device.index, kw_id, wkey)
-        if key not in self._graphs:
-            z_in = torch.empty(x_T.shape, dtype=torch.float32, device=x_T.device)
-            x, den = torch.empty_like(z_in), torch.empty_like(z_in)
-
-            def warmup():
-                x.copy_(x_T)
-                self._run(x, den, ts, model_kwargs)
-
-            def body():
-                x.copy_(z_in)
-                self._run(x, den, ts, model_kwargs)
-            self._graphs[key] = (_capture(warmup, body), z_in, den, ts)
-        graph, z_in, den = self._graphs[key][:3]
-        z_in.copy_(x_T)
-        graph.replay()
-        return den.clone()
+        if cuda_graph:                                     # the timestep is fixed per sampler: no extras in the key
+            return self._graphs.sample(self.model, model_kwargs, (), x_T, None, loop, (ts,))
+        return loop(x_T, None, None)
 
 
 # ================================================================================================= distillation
@@ -281,7 +264,7 @@ class DMDDistiller:
         # mse(out[:, :4], target) and its gradient: the L2 consistency loss over a row that makes model_pred = eps and the
         # target = x_prev exactly (cskip_s 0, cout_s 1, sra_s 0, srm1_s -1; cskip_t 1, cout_t 0); ema_out is multiplied by 0
         index = self._workspace(out.shape[0])[2]
-        return _ConsistencyLoss.apply(out, _step_input(out.detach()), target, target, index, self._mse_table,
+        return _ConsistencyLoss.apply(out, step_input(out.detach()), target, target, index, self._mse_table,
                                       self._mse_partials, lib.LCM_L2, 1.0)
 
     def step(self, y: torch.Tensor, mask: Optional[torch.Tensor] = None, data_info=None, draws=None,
@@ -316,7 +299,7 @@ class DMDDistiller:
             out_g = out_g.float()
         with torch.no_grad():
             latents, scratch = torch.empty_like(init_noise), torch.empty_like(init_noise)
-            lib.lcm_step(_step_input(out_g[:, :4]), init_noise, None, latents, scratch, **self.gen_scalars)
+            lib.lcm_step(step_input(out_g[:, :4]), init_noise, None, latents, scratch, **self.gen_scalars)
             noisy = self.add_noise(latents, noise.to(latents.device), t).contiguous()
             # 2. the real model at batch 2b over [uncond ; cond]
             uy = self.uncond_y.to(dtype=y.dtype).expand(b, *self.uncond_y.shape[1:])
@@ -327,7 +310,7 @@ class DMDDistiller:
         # the fake model's score: on the training path (the fp32 master is not an inference model), detached
         ag.refresh_shadows(self.fake)
         fake_out = self.fake(noisy, t, y, mask=mask, data_info=di).detach()
-        dm = _DmdLoss.apply(out_g, latents, noisy, t, self.ac, _step_input(real_out), _step_input(fake_out), partials, weight,
+        dm = _DmdLoss.apply(out_g, latents, noisy, t, self.ac, step_input(real_out), step_input(fake_out), partials, weight,
                             self.cfg, self.gen_scalars["sqrt_alpha"], self.gen_scalars["sqrt_beta"])
         (dm * loss_scale if loss_scale != 1.0 else dm).backward()
         del fake_out, real_out

@@ -12,6 +12,7 @@ from typing import Dict, Optional, Tuple
 
 import torch
 
+from .capture import capture_graph, kwargs_key, weights_key
 from .lora import require_merged as require_lora_merged
 
 
@@ -27,33 +28,18 @@ class GraphedForward:
             raise ValueError(f"GraphedForward supports {self.METHODS}, got {method!r}")
         self.model, self.method = model, method
         self._graphs: Dict[Tuple, dict] = {}
-        self._params = list(model.parameters())
         self._wkey = None
-
-    @staticmethod
-    def _key(x, y, mask, data_info):
-        di = None
-        if data_info is not None:
-            di = tuple(sorted((k, (v.data_ptr(), tuple(v.shape)) if isinstance(v, torch.Tensor) else repr(v))
-                              for k, v in data_info.items()))
-        return (tuple(x.shape), tuple(y.shape), None if mask is None else tuple(mask.shape), di)
 
     @torch.no_grad()
     def __call__(self, x: torch.Tensor, timestep: torch.Tensor, y: torch.Tensor, mask: Optional[torch.Tensor] = None,
                  data_info=None) -> torch.Tensor:
         require_lora_merged(self.model)           # a graph captured before an adapter was attached would ignore it
-        dev = self._params[0].device
-        # The kernels read the parameters in place, but the fused-LN forward also keeps tables derived from them
-        # that a captured graph cannot refresh: an in-place update or a re-assignment of any parameter (optimizer / EMA step,
-        # .to(dtype)) drops the captured graphs.
-        # (Without such copies -- the default configuration -- a replay reads the updated parameters in place and nothing is dropped.)
-        wkey = (sum(p._version for p in self._params), self._params[0].data_ptr(), self._params[-1].data_ptr())
+        dev = next(self.model.parameters()).device
+        wkey = weights_key(self.model)                 # changes only when a replay could not see the parameters' update
         if wkey != self._wkey:
-            derived = getattr(self.model, "_ln_fusion", None) is not None
-            if self._wkey is not None and derived:
-                self._graphs.clear()
+            self._graphs.clear()
             self._wkey = wkey
-        key = self._key(x, y, mask, data_info)
+        key = (tuple(x.shape), tuple(y.shape), None if mask is None else tuple(mask.shape), kwargs_key(data_info))
         g = self._graphs.get(key)
         if g is None:
             st = {"x": torch.empty(x.shape, dtype=torch.float32, device=dev),
@@ -66,15 +52,8 @@ class GraphedForward:
                 call = lambda: fn(st["x"], st["t"], st["y"], mask=st["mask"], data_info=data_info)
             else:
                 call = lambda: fn(st["x"], st["t"], st["y"], data_info=data_info, mask=st["mask"])
-            side = torch.cuda.Stream(device=dev)
-            side.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(side):
-                for _ in range(2):                      # eager warm-up: sizes the workspace, fills caches
-                    call()
-            torch.cuda.current_stream(dev).wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                out = call()
+            # two eager warm-up calls: size the workspace, fill caches
+            graph, out = capture_graph(lambda: (call(), call()), call, dev)
             g = {"graph": graph, "static": st, "out": out}
             self._graphs[key] = g
         self._copy_in(g["static"], x, timestep, y, mask)

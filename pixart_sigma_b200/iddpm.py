@@ -26,15 +26,14 @@ per-step generator on any device), pinned against the unmodified reference sampl
 """
 from __future__ import annotations
 
-import time
 from typing import Callable, Dict, Iterator, List, Optional, Sequence
 
 import numpy as np
 import torch
 
 from . import lib
+from .capture import CapturedLoops, step_input
 from .model import PixArt, PixArtMS
-from .sampler import _capture, _denoiser_key, _denoiser_params
 
 # pxa_iddpm_step scalar -> IDDPMSampler.tab entry it is read from (p_mean_variance's _extract_into_tensor calls)
 _STEP_TABLES = (("sqrt_recip_ac", "sqrt_recip_ac"), ("sqrt_recipm1_ac", "sqrt_recipm1_ac"), ("post_c1", "post_c1"),
@@ -99,8 +98,9 @@ class IDDPMSampler:
         self._dev: Dict[str, torch.Tensor] = {}
         self._plan: Optional[List[dict]] = None
         self._tmaps: Dict[tuple, torch.Tensor] = {}
-        self._graphs: Dict[tuple, tuple] = {}
-        self.last_capture_s: Optional[float] = None          # wall time of the latest CUDA-graph capture (cuda_graph=True)
+        self._graphs = CapturedLoops()
+
+    last_capture_s = property(lambda self: self._graphs.last_capture_s)    # wall time of the latest CUDA-graph capture
 
     def _x(self, name: str, t: torch.Tensor) -> torch.Tensor:                 # _extract_into_tensor, :1029-1041
         key = f"{name}@{t.device}"
@@ -216,19 +216,27 @@ class IDDPMSampler:
         if tuple(x_T.shape) != size:
             raise ValueError(f"noise must have shape {size}")
         t_all = self._timesteps(device, size[0])
+
+        def loop(x0, k, draws):
+            img = x0.to(torch.float32).contiguous().clone()
+            inp = _first_input(img) if guided else None
+            zbuf = torch.empty_like(img) if draws is None else None
+            return self._run(fwd, img, inp, zbuf, plan[:k], t_all[:k], guided, cfg, clip, draws)
         if cuda_graph:
-            return self._sample_graphed(model, model_kwargs, fwd, x_T, plan, t_all, guided, cfg, clip, noise_draws)
-        img = x_T.to(torch.float32).contiguous().clone()
-        inp = _first_input(img) if guided else None
-        zbuf = torch.empty_like(img) if noise_draws is None else None
-        return self._run(fwd, img, inp, zbuf, plan, t_all, guided, cfg, clip, noise_draws)
+            extras = (guided, cfg, bool(clip), tuple(st["map_t"] for st in plan))
+            return self._graphs.sample(model, model_kwargs, extras, x_T, noise_draws, loop, (t_all,))
+        return loop(x_T, None, noise_draws)
 
     @staticmethod
     def _run(fwd, img, inp, zbuf, plan, t_all, guided, cfg, clip, draws):
         """All steps, in place on img (and, guided, on the model input inp).  draws None: each step draws into zbuf from the
         default generator after its forward, as p_sample draws after p_mean_variance; otherwise draws[k] is step k's."""
+        N, C, h, w = img.shape
         for k, st in enumerate(plan):
-            out = _step_input(fwd(inp if guided else img, t_all[k]), img.shape)
+            out = fwd(inp if guided else img, t_all[k])
+            if tuple(out.shape) != (N, 2 * C, h, w):
+                raise ValueError(f"the model returned {tuple(out.shape)}, expected {(N, 2 * C, h, w)} (eps and learned variance)")
+            out = step_input(out, fp16=True)
             if draws is None:
                 zbuf.normal_()
                 z = zbuf
@@ -237,51 +245,6 @@ class IDDPMSampler:
             lib.iddpm_step(out, img, z if st["t"] != 0 else None, inp, guided=guided, clip=clip, cfg_scale=cfg,
                            **{key: st[key] for key in _STEP_KEYS})
         return img
-
-    def _sample_graphed(self, model, model_kwargs, fwd, x_T, plan, t_all, guided, cfg, clip, draws):
-        # the scalars, the timestep tensors and the model_kwargs tensors are captured by address or value: all in the key
-        owner = getattr(model, "__self__", model)
-        params = _denoiser_params(model)
-        dtypes = (getattr(owner, "output_dtype", None), params[0].dtype if params else None)   # the captured forward's path
-        kw_id, wkey = _denoiser_key(model, params, model_kwargs)
-        key = (tuple(x_T.shape), x_T.device.index, id(owner), getattr(model, "__func__", None), guided, cfg, bool(clip),
-               tuple(st["map_t"] for st in plan), kw_id, wkey, dtypes, draws is None)
-        if key not in self._graphs:
-            z_in = torch.empty(x_T.shape, dtype=torch.float32, device=x_T.device)
-            img, zbuf = torch.empty_like(z_in), torch.empty_like(z_in)
-            inp = torch.empty_like(z_in) if guided else None
-            draws_in = None if draws is None else torch.zeros((len(plan),) + tuple(z_in.shape), device=z_in.device)
-            zeros = [torch.zeros_like(z_in)] * 2
-
-            def load():
-                img.copy_(z_in)
-                if guided:
-                    n = z_in.shape[0] // 2
-                    inp[:n].copy_(z_in[:n])
-                    inp[n:].copy_(z_in[:n])
-
-            def warmup():                                  # replayed-noise form: consumes no random numbers
-                z_in.copy_(x_T)
-                load()
-                self._run(fwd, img, inp, zbuf, plan[:2], t_all[:2], guided, cfg, clip, zeros)
-
-            def body():
-                load()
-                self._run(fwd, img, inp, zbuf, plan, t_all, guided, cfg, clip,
-                          None if draws_in is None else draws_in.unbind(0))
-            t0 = time.perf_counter()
-            graph = _capture(warmup, body)
-            torch.cuda.synchronize(x_T.device)
-            self.last_capture_s = time.perf_counter() - t0
-            # the model and its kwargs are kept alive with the graph: their tensors are captured by address
-            self._graphs[key] = (graph, z_in, img, draws_in, t_all, model, model_kwargs)
-        graph, z_in, img, draws_in = self._graphs[key][:4]
-        z_in.copy_(x_T)
-        if draws_in is not None:
-            for dst, src in zip(draws_in.unbind(0), draws):
-                dst.copy_(src)
-        graph.replay()
-        return img.clone()
 
 
 def _native_cfg_owner(model: Callable) -> Optional[PixArtMS]:
@@ -309,18 +272,6 @@ def _denoiser(model: Callable, owner: Optional[PixArtMS], model_kwargs: Optional
 def _first_input(img: torch.Tensor) -> torch.Tensor:
     half = img[: img.shape[0] // 2]
     return torch.cat([half, half]).contiguous()
-
-
-def _step_input(out: torch.Tensor, shape) -> torch.Tensor:
-    """The model output as pxa_iddpm_step reads it: (N, 8, h, w) fp32 / bf16 / fp16 with dense (h, w) planes."""
-    N, C, h, w = shape
-    if tuple(out.shape) != (N, 2 * C, h, w):
-        raise ValueError(f"the model returned {tuple(out.shape)}, expected {(N, 2 * C, h, w)} (eps and learned variance)")
-    if out.dtype not in (torch.float32, torch.bfloat16, torch.float16):
-        out = out.float()
-    if not (out.stride(3) == 1 and out.stride(2) == w and out.stride(1) == h * w):
-        out = out.contiguous()
-    return out
 
 
 def IDDPM(timestep_respacing, noise_schedule: str = "linear", use_kl: bool = False, sigma_small: bool = False,

@@ -25,7 +25,7 @@ import numpy as np
 import torch
 
 from . import lib
-from .sampler import _capture, _denoiser_key, _denoiser_params, _step_input
+from .capture import CapturedLoops, step_input
 from .training import IDDPMLoss
 
 __all__ = ["LCMScheduler", "LCMSchedulerOutput", "LCMSampler", "LCMDistiller", "GraphedLCMStep", "FlatEMA",
@@ -124,7 +124,7 @@ class LCMScheduler:
         if len(self.timesteps) > 1:
             noise = torch.randn(model_output.shape).to(model_output.device)
         denoised, prev = torch.empty_like(x), torch.empty_like(x)
-        lib.lcm_step(_step_input(model_output), x, noise, denoised, prev, **st)
+        lib.lcm_step(step_input(model_output), x, noise, denoised, prev, **st)
         if not return_dict:
             return prev, denoised
         return LCMSchedulerOutput(prev_sample=prev, denoised=denoised)
@@ -138,9 +138,8 @@ class LCMSampler:
     def __init__(self, model_fn: Callable, **scheduler_kwargs):
         self.model = model_fn
         self.scheduler = LCMScheduler(**scheduler_kwargs)
-        self._params = _denoiser_params(model_fn)
         self._plans: Dict[tuple, List[dict]] = {}
-        self._graphs: Dict[tuple, tuple] = {}
+        self._graphs = CapturedLoops()
 
     def plan(self, steps: int, lcm_origin_steps: int = 50) -> List[dict]:
         """Per step: the int64 timestep and the scalars of `pxa_lcm_step`."""
@@ -165,7 +164,7 @@ class LCMSampler:
     def _run(self, x, denoised, plan, ts_dev, noise, model_kwargs):
         for i, (st, ts) in enumerate(zip(plan, ts_dev)):
             out = self.model(x, ts, **model_kwargs)
-            lib.lcm_step(_step_input(out[:, :4]), x, noise[i] if st["c_noise"] != 0.0 else None, denoised, x,
+            lib.lcm_step(step_input(out[:, :4]), x, noise[i] if st["c_noise"] != 0.0 else None, denoised, x,
                          **{k: st[k] for k in ("sqrt_alpha", "sqrt_beta", "c_skip", "c_out", "c_prev", "c_noise")})
         return denoised
 
@@ -195,36 +194,15 @@ class LCMSampler:
             noise = None
         n = shape[0]
         ts_dev = [torch.full((n,), st["t"], dtype=torch.int64, device=x_T.device) for st in plan]
+
+        def loop(x0, k, draws):
+            x = x0.to(torch.float32).contiguous().clone()
+            return self._run(x, torch.empty_like(x), plan[:k], ts_dev[:k], draws, model_kwargs)
         if cuda_graph:
-            return self._sample_graphed(x_T, plan, ts_dev, noise, model_kwargs)
-        x = x_T.to(torch.float32).contiguous().clone()
-        return self._run(x, torch.empty_like(x), plan, ts_dev, noise, model_kwargs)
-
-    def _sample_graphed(self, x_T, plan, ts_dev, noise, model_kwargs):
-        # the step scalars and timesteps are baked into the captured launches, model_kwargs tensors and the parameters
-        # (through derived weight copies) into the captured forward: all are part of the key
-        kw_id, wkey = _denoiser_key(self.model, self._params, model_kwargs)
-        key = (tuple(x_T.shape), x_T.device.index, kw_id, wkey, tuple(tuple(sorted(st.items())) for st in plan))
-        if key not in self._graphs:
-            z_in = torch.empty(x_T.shape, dtype=torch.float32, device=x_T.device)
-            x, den = torch.empty_like(z_in), torch.empty_like(z_in)
-            noise_in = None if noise is None else torch.zeros_like(noise)
-
-            def warmup():
-                x.copy_(x_T)
-                self._run(x, den, plan[:2], ts_dev[:2], noise_in, model_kwargs)
-
-            def body():
-                x.copy_(z_in)
-                self._run(x, den, plan, ts_dev, noise_in, model_kwargs)
-            graph = _capture(warmup, body)
-            self._graphs[key] = (graph, z_in, den, noise_in, ts_dev)
-        graph, z_in, den, noise_in = self._graphs[key][:4]
-        z_in.copy_(x_T)
-        if noise_in is not None:
-            noise_in.copy_(noise)
-        graph.replay()
-        return den.clone()
+            # the step scalars and timesteps are baked into the captured launches
+            extras = (tuple(tuple(sorted(st.items())) for st in plan),)
+            return self._graphs.sample(self.model, model_kwargs, extras, x_T, noise, loop, (ts_dev,))
+        return loop(x_T, None, noise)
 
 
 # ================================================================================================= distillation
@@ -451,10 +429,10 @@ class LCMDistiller:
                                                   for k, v in data_info.items()}
             out_t = self.teacher(torch.cat([x_t, x_t]), torch.cat([start, start]), torch.cat([y, uncond]), mask=m2, data_info=di2)
             x_prev = torch.empty_like(x_t)
-            lib.lcm_teacher_target(_step_input(out_t), x_t, index, self.table, x_prev, w=self.w)
+            lib.lcm_teacher_target(step_input(out_t), x_t, index, self.table, x_prev, w=self.w)
             _check_ema_forward(self.ema, "LCMDistiller")
             out_e = self.ema(x_prev, t, y, mask=mask, data_info=data_info)
-        return _ConsistencyLoss.apply(out_s, _step_input(out_e), x_t, x_prev, index, self.table, self.partials, self.loss_type,
+        return _ConsistencyLoss.apply(out_s, step_input(out_e), x_t, x_prev, index, self.table, self.partials, self.loss_type,
                                       self.huber_c)
 
     def step(self, latents: torch.Tensor, y: torch.Tensor, mask: Optional[torch.Tensor] = None, data_info=None,

@@ -24,7 +24,8 @@ from typing import Callable, Dict, List, Optional, Sequence
 import torch
 
 from . import lib
-from .sampler import _DiscreteVPSchedule, _capture, _denoiser_key, _denoiser_params, _step_input, linear_betas
+from .capture import CapturedLoops, CfgCond, step_input
+from .sampler import _DiscreteVPSchedule, linear_betas
 
 __all__ = ["SASolverSampler"]
 
@@ -56,10 +57,9 @@ class SASolverSampler:
         # float64 cumprod cast to float32, then 0.5 * log in float32 (diffusion/sa_sampler.py:19-22, sa_solver.py:86)
         alphas_cumprod = torch.cumprod(1.0 - torch.from_numpy(linear_betas(diffusion_steps)), dim=0).to(torch.float32)
         self.schedule = _DiscreteVPSchedule(log_alpha=0.5 * torch.log(alphas_cumprod))
-        self._params = _denoiser_params(model)
         self._plans: Dict[tuple, List[dict]] = {}
-        self._graphs: Dict[tuple, tuple] = {}
-        self._cfg_cond: Optional[tuple] = None             # (key, cat([uncond, cond])), rebuilt when either input changes
+        self._graphs = CapturedLoops()
+        self._cfg_cond = CfgCond()
 
     # ---- host side: everything that does not depend on the latents
     def _update(self, ts: torch.Tensor, i: int, order: int, tau, corrector: bool):
@@ -131,17 +131,10 @@ class SASolverSampler:
             else:
                 cur, nxt = (noise[i - 1] if i else None), noise[i]
             out = self.model(torch.cat([x_pred, x_pred]) if guided else x_pred, t_in, cond, **model_kwargs)
-            lib.sa_solver_step(_step_input(out), x, x_pred, m_prev, cur if st["c_noise"] else None,
+            lib.sa_solver_step(step_input(out), x, x_pred, m_prev, cur if st["c_noise"] else None,
                                nxt if st["p_noise"] else None, guided=guided, cfg_scale=cfg,
                                **{k: st[k] for k in _STEP_KEYS})
         return x_pred
-
-    def _cond(self, conditioning, unconditional_conditioning):
-        key = tuple((t.data_ptr(), t._version, tuple(t.shape), t.dtype) for t in (unconditional_conditioning, conditioning))
-        if self._cfg_cond is None or self._cfg_cond[0] != key:
-            # [uncond ; cond] (sa_solver.py:316), built once per input pair so that a captured loop can be replayed
-            self._cfg_cond = (key, torch.cat([unconditional_conditioning, conditioning]))
-        return self._cfg_cond[1]
 
     @torch.no_grad()
     def sample(self, S, batch_size, shape, conditioning=None, callback=None, normals_sequence=None, img_callback=None,
@@ -176,51 +169,21 @@ class SASolverSampler:
             x_T = torch.randn(size, device=device)                       # sa_sampler.py:70-71
         elif tuple(x_T.shape) != size:
             raise ValueError(f"x_T must have shape {size}")
-        cond = self._cond(conditioning, unconditional_conditioning) if guided else conditioning
+        cond = self._cfg_cond(unconditional_conditioning, conditioning) if guided else conditioning     # sa_solver.py:316
         cfg = float(unconditional_guidance_scale) if guided else 1.0
         rows = 2 * batch_size if guided else batch_size
         t_dev = [torch.full((rows,), st["t_input"], dtype=torch.float32, device=device) for st in plan]
-        if cuda_graph:
-            out = self._sample_graphed(x_T, plan, t_dev, cond, guided, cfg, model_kwargs, noise)
-        else:
-            x = x_T.to(torch.float32).contiguous().clone()
+
+        def loop(x0, k, draws):
+            x = x0.to(torch.float32).contiguous().clone()
             x_pred = x.clone()
             m_prev, bufs = torch.empty_like(x), [torch.empty_like(x), torch.empty_like(x)]
-            out = self._run(x, x_pred, m_prev, bufs, plan, t_dev, cond, guided, cfg, model_kwargs, noise)
+            return self._run(x, x_pred, m_prev, bufs, plan[:k], t_dev[:k], cond, guided, cfg, model_kwargs, draws)
+        if cuda_graph:
+            # the per-evaluation scalars and t_input are baked into the captured kernel arguments
+            extras = (guided, cfg, cond.data_ptr(), tuple(cond.shape),
+                      tuple(tuple(st[k] for k in ("t_input",) + _STEP_KEYS) for st in plan))
+            out = self._graphs.sample(self.model, model_kwargs, extras, x_T, noise, loop, (cond, t_dev))
+        else:
+            out = loop(x_T, None, noise)
         return out.to(x_T.dtype), None
-
-    def _sample_graphed(self, x_T, plan, t_dev, cond, guided, cfg, model_kwargs, noise):
-        # the per-evaluation scalars and t_input are baked into the captured kernel arguments, and `cond` / model_kwargs
-        # tensors into the captured forward: all of them are part of the key
-        kw_id, wkey = _denoiser_key(self.model, self._params, model_kwargs)
-        key = (tuple(x_T.shape), x_T.device.index, guided, cfg, cond.data_ptr(), tuple(cond.shape), kw_id, wkey,
-               noise is None, tuple(tuple(st[k] for k in ("t_input",) + _STEP_KEYS) for st in plan))
-        if key not in self._graphs:
-            z_in = torch.empty(x_T.shape, dtype=torch.float32, device=x_T.device)
-            x, x_pred, m_prev = torch.empty_like(z_in), torch.empty_like(z_in), torch.empty_like(z_in)
-            bufs = [torch.empty_like(z_in), torch.empty_like(z_in)]
-            noise_in = None if noise is None else torch.zeros((len(plan),) + tuple(z_in.shape), device=z_in.device)
-            zeros = [torch.zeros_like(z_in)] * len(plan)
-
-            def load():
-                x.copy_(z_in)
-                x_pred.copy_(z_in)
-
-            def warmup():                                  # replayed-noise form: consumes no random numbers
-                z_in.copy_(x_T)
-                load()
-                self._run(x, x_pred, m_prev, bufs, plan[:2], t_dev[:2], cond, guided, cfg, model_kwargs, zeros)
-
-            def body():
-                load()
-                self._run(x, x_pred, m_prev, bufs, plan, t_dev, cond, guided, cfg, model_kwargs,
-                          None if noise_in is None else noise_in.unbind(0))
-            graph = _capture(warmup, body)
-            self._graphs[key] = (graph, z_in, x_pred, noise_in, t_dev, cond)
-        graph, z_in, x_pred, noise_in = self._graphs[key][:4]
-        z_in.copy_(x_T)
-        if noise_in is not None:
-            for dst, src in zip(noise_in.unbind(0), noise):
-                dst.copy_(src)
-        graph.replay()
-        return x_pred.clone()

@@ -16,12 +16,13 @@ There is no CPU path: inputs must live on an sm_90 device.
 """
 from __future__ import annotations
 
-from typing import Callable, Dict, List, Optional
+from typing import Callable, List, Optional
 
 import numpy as np
 import torch
 
 from . import lib
+from .capture import CapturedLoops, CfgCond, step_input
 
 __all__ = ["DPMS", "DPMSolverPP"]
 
@@ -30,44 +31,6 @@ def linear_betas(diffusion_steps: int = 1000) -> np.ndarray:
     """float64 linear beta schedule (diffusion/model/gaussian_diffusion.py:82,107-116)."""
     scale = 1000 / diffusion_steps
     return np.linspace(scale * 0.0001, scale * 0.02, diffusion_steps, dtype=np.float64)
-
-
-def _denoiser_params(model: Callable) -> list:
-    owner = getattr(model, "__self__", model)              # the nn.Module behind a bound forward_with_dpmsolver
-    return list(owner.parameters()) if isinstance(owner, torch.nn.Module) else []
-
-
-def _denoiser_key(model: Callable, params: list, model_kwargs: Optional[dict]) -> tuple:
-    """The denoiser's part of a captured sampling loop's cache key.  `model_kwargs` tensors are captured by address, and so
-    are the denoiser's parameters: the fused-LN forward keeps tables derived from them that a replay cannot refresh."""
-    kw_id = tuple(sorted((k, (v.data_ptr(), tuple(v.shape)) if isinstance(v, torch.Tensor) else repr(v))
-                         for k, v in (model_kwargs or {}).items()))
-    owner = getattr(model, "__self__", model)
-    derived = getattr(owner, "_ln_fusion", None) is not None
-    wkey = (sum(p._version for p in params), params[0].data_ptr()) if (params and derived) else None
-    return kw_id, wkey
-
-
-def _capture(warmup: Callable[[], None], body: Callable[[], None]) -> torch.cuda.CUDAGraph:
-    """Run `warmup` eagerly on a side stream (lazy inits, tensor maps), then capture `body` into a CUDA graph."""
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        warmup()
-    torch.cuda.current_stream().wait_stream(side)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        body()
-    return graph
-
-
-def _step_input(out: torch.Tensor) -> torch.Tensor:
-    """The denoiser output as a step kernel reads it: fp32 or bf16 with dense (h, w) planes (channel slices are fine)."""
-    if out.dtype not in (torch.float32, torch.bfloat16):
-        out = out.float()
-    if not (out.stride(3) == 1 and out.stride(2) == out.shape[3] and out.stride(1) == out.shape[2] * out.shape[3]):
-        out = out.contiguous()
-    return out
 
 
 class _DiscreteVPSchedule:
@@ -117,9 +80,8 @@ class DPMSolverPP:
         self.cfg_scale = float(cfg_scale)
         self.model_kwargs = dict(model_kwargs or {})
         self.schedule = _DiscreteVPSchedule(diffusion_steps)
-        self._graphs: Dict[tuple, tuple] = {}
-        self._cfg_cond: Optional[torch.Tensor] = None          # cat([uncondition, condition]), built once
-        self._params = _denoiser_params(model)
+        self._graphs = CapturedLoops()
+        self._cfg_cond = CfgCond()
 
     # ---- host side: everything that does not depend on the latents
     def plan(self, steps: int, order: int = 2, t_start: Optional[float] = None, t_end: Optional[float] = None,
@@ -158,7 +120,7 @@ class DPMSolverPP:
             else:                                   # reference: a single conditional evaluation (dpm_solver.py:327-328)
                 out = self.model(x, t_in[:n], cond, **self.model_kwargs)
                 out = torch.cat([out, out])
-            lib.dpm_solver_pp_step(_step_input(out), x, x0_prev, cfg_scale=self.cfg_scale if guided else 1.0,
+            lib.dpm_solver_pp_step(step_input(out), x, x0_prev, cfg_scale=self.cfg_scale if guided else 1.0,
                                    sigma_s=st["sigma_s"], alpha_s=st["alpha_s"], a=st["a"], b=st["b"], c=st["c"])
             if inter is not None:
                 inter.append(x.clone())
@@ -179,39 +141,21 @@ class DPMSolverPP:
         plan = self.plan(steps, order, t_start, t_end, lower_order_final)
         n = x.shape[0]
         guided = self.uncondition is not None and self.cfg_scale != 1.
-        if guided and self._cfg_cond is None:
-            self._cfg_cond = torch.cat([self.uncondition, self.condition])    # [uncond ; cond] (dpm_solver.py:330)
-        cond = self._cfg_cond if guided else self.condition
+        cond = self._cfg_cond(self.uncondition, self.condition) if guided else self.condition    # dpm_solver.py:330
         t_dev = [torch.full((2 * n,), st["t_input"], dtype=torch.float32, device=x.device) for st in plan]
-        if cuda_graph and not return_intermediate:
-            return self._sample_graphed(x, plan, t_dev, cond)
-        xs = x.to(torch.float32).contiguous().clone()
-        x0_prev = torch.empty_like(xs)
         inter = [] if return_intermediate else None
-        out = self._run(xs, x0_prev, plan, t_dev, cond, inter)
+
+        def loop(x0, k, draws):
+            xs = x0.to(torch.float32).contiguous().clone()
+            return self._run(xs, torch.empty_like(xs), plan[:k], t_dev[:k], cond, inter)
+        if cuda_graph and not return_intermediate:
+            # every per-step scalar, the step orders and t_input are baked into the captured kernel arguments
+            extras = (self.cfg_scale, cond.data_ptr(), tuple(cond.shape), tuple(tuple(st.values()) for st in plan))
+            out = self._graphs.sample(self.model, self.model_kwargs, extras, x, None, loop, (cond, t_dev))
+        else:
+            out = loop(x, None, None)
         out = out.to(x.dtype)
         return (out, inter) if return_intermediate else out
-
-    def _sample_graphed(self, x, plan, t_dev, cond):
-        # every per-step scalar (sigma_s, alpha_s, a, b, c), the step orders and t_input are baked into the captured kernel
-        # arguments, and `cond` / model_kwargs tensors into the captured forward: all of them are part of the key
-        kw_id, wkey = _denoiser_key(self.model, self._params, self.model_kwargs)
-        key = (tuple(x.shape), x.device.index, float(self.cfg_scale), cond.data_ptr(), tuple(cond.shape), kw_id, wkey,
-               tuple((st["t_input"], st["sigma_s"], st["alpha_s"], st["a"], st["b"], st["c"], st.get("order")) for st in plan))
-        if key not in self._graphs:
-            x_static = x.to(torch.float32).contiguous().clone()
-            x0_prev = torch.empty_like(x_static)
-            z_in = torch.empty_like(x_static)
-
-            def body():
-                x_static.copy_(z_in)
-                self._run(x_static, x0_prev, plan, t_dev, cond, None)
-            graph = _capture(lambda: self._run(x_static, x0_prev, plan[:2], t_dev[:2], cond, None), body)
-            self._graphs[key] = (graph, z_in, x_static, t_dev, cond)
-        graph, z_in, x_static = self._graphs[key][:3]
-        z_in.copy_(x)
-        graph.replay()
-        return x_static.to(x.dtype).clone()
 
 
 def DPMS(model: Callable, condition: torch.Tensor, uncondition: Optional[torch.Tensor], cfg_scale: float,
