@@ -130,6 +130,59 @@ typedef struct PxaGemmTail {
 } PxaGemmTail;
 int pxa_gemm_lora_bf16(const PxaGemmArgs* args, const PxaGemmTail* tail, void* stream);
 
+/* ------------------------------------------------------------------------------------------- DoRA (weight-decomposed LoRA)
+ * A DoRA projection computes y = c . (x W^T + s (x A^T) B^T) + bias with c[n] = m[n] / ||W[n,:] + s (B A)[n,:]||_2 per output
+ * row: m is the trained fp32 magnitude, the norm is taken without gradient (DoRA paper, section 4.3).
+ *
+ * pxa_gemm_dora_bf16: out = epilogue( col_scale[n] * (A W^T [+ tail_a tail_w^T]) + bias ).  The scale multiplies the fp32
+ * accumulator before anything else: EPI_BIAS_GELU_AUX keeps c acc + bias as the pre-activation and EPI_BIAS_RESIDUAL with
+ * aux_is_branch writes c acc + bias to the aux copy.  tail may be NULL.  Takes K-major operands and EPI_BIAS, EPI_BIAS_GELU,
+ * EPI_BIAS_GELU_AUX and EPI_BIAS_RESIDUAL (gate and aux included); every other form, aux_scale and row_stats_out return
+ * PXA_ERR_ARG.  col_scale: fp32 [N], 4-byte aligned.  Block widths as pxa_gemm_lora_bf16 with a tail, pxa_gemm_bf16 without. */
+int pxa_gemm_dora_bf16(const PxaGemmArgs* args, const PxaGemmTail* tail, const float* col_scale, void* stream);
+
+/* pxa_dora_norm: wn[n] = || W[n,:] + (b a)[n,:] ||_2 and c[n] = m[n] / wn[n] in fp32 for n_items same-shaped projections.
+ * W is the bf16 weight the forward GEMM multiplies; a [T, K] and b [N, T] are the bf16 adapter operands that GEMM's K-tail
+ * reads (a = A with zero rows past G r, b = s blockdiag(B)), so wn is the norm of the weight the tail-extended GEMM applies.
+ * Against the fp32 s B A, each element of b a differs by at most 2^-8 (2 + 2^-8) sum_t |b[n,t] a[t,k]| (two bf16 roundings).
+ * One fixed-order reduction per row: deterministic, and wn of B = 0 with m = wn gives c = 1 exactly.  Items are launched 64
+ * at a time; n_items <= 0 is a no-op.  N, K multiples of 8, T a multiple of 8 and <= 256 (PXA_ERR_ARG). */
+typedef struct PxaDoraNormItem {
+  const void* w;        /* bf16 [N, K] contiguous                                        */
+  const void* a;        /* bf16 [T, K] contiguous                                        */
+  const void* b;        /* bf16 [N, T] contiguous                                        */
+  const float* m;       /* fp32 [N] magnitude, or NULL (then c must be NULL)             */
+  float* wn;            /* fp32 [N] written, or NULL                                     */
+  float* c;             /* fp32 [N] written: m / wn, or NULL                             */
+} PxaDoraNormItem;
+typedef struct PxaDoraNormArgs {
+  const PxaDoraNormItem* items;   /* host array of n_items */
+  int32_t n_items;
+  int32_t N, K, T;
+} PxaDoraNormArgs;
+int pxa_dora_norm(const PxaDoraNormArgs* args, void* stream);
+
+/* pxa_dora_bwd: the DoRA part of a projection's backward, from g = dL/dy (y = c z + bias, the projection's output before any
+ * activation / gate) and the saved y:
+ *   dz = bf16(c . g)                                 (dz may alias g; it feeds the unchanged dgrad / adapter passes)
+ *   dm[n] += sum_r g[r,n] (y[r,n] - bias[n]) / m[n]  (= sum_r g z / wn; m must be non-zero)
+ * The row sum runs in fixed order: per-chunk partials of PXA_DORA_BWD_ROWS rows, then one ordered sum per column (no float
+ * atomics, two launches; the same inputs give the same bits).  N a multiple of 8; ldg / ldy / ldz multiples of 8. */
+#define PXA_DORA_BWD_ROWS 128
+typedef struct PxaDoraBwdArgs {
+  const void* g;        /* bf16 [M, N], row stride ldg                                                   */
+  const void* y;        /* bf16 [M, N], row stride ldy                                                   */
+  const void* bias;     /* bf16 [N] or NULL                                                              */
+  const float* c;       /* fp32 [N]                                                                      */
+  const float* m;       /* fp32 [N]                                                                      */
+  void* dz;             /* bf16 [M, N], row stride ldz (may alias g with ldz == ldg)                     */
+  float* dm;            /* fp32 [N], accumulated                                                         */
+  float* partials;      /* fp32 workspace of ceil(M / PXA_DORA_BWD_ROWS) * N floats                      */
+  int64_t ldg, ldy, ldz;
+  int32_t M, N;
+} PxaDoraBwdArgs;
+int pxa_dora_bwd(const PxaDoraBwdArgs* args, void* stream);
+
 /* ------------------------------------------------------------------------------------ LayerNorm + modulate
  * out[r,:] = LN(x[r,:]; eps, no affine) * (1 + scale[b,:]) + shift[b,:]  with b = r / rows_per_batch, bf16 out.
  * Replaces norm1/norm2 + t2i_modulate (PixArtMS.py:58,64,75,77; PixArt_blocks.py:24-25) and the final-layer

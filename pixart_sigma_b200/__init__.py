@@ -12,7 +12,7 @@ Only what the path `PixArtMS.forward -> 28 x PixArtMSBlock.forward` needs:
   lcm.py     LCM: the few-step sampler (mirror of the reference's `LCMScheduler` loop) and consistency distillation with a
              fused flat EMA update
   dmd.py     DMD: distribution-matching distillation to a one-step generator (fused loss kernel) and one-step sampling
-  lora.py    LoRA adapters in peft's directory format, merged into the weights for sampling
+  lora.py    LoRA and DoRA adapters in peft's directory format, merged into the weights for sampling
   autograd.py / training.py  training path: the block's ops as autograd Functions over forward + backward kernels, IDDPM loss
   parallel.py  batch-sharded inference replicas; bucketed gradient all-reduce for data-parallel training
   vae.py / t5.py  the callers either side of the path on the same kernels: SDXL-VAE (diffusers' AutoencoderKL layout) and the
@@ -23,7 +23,8 @@ Only what the path `PixArtMS.forward -> 28 x PixArtMSBlock.forward` needs:
 from .model import (MODELS, PixArt, PixArt_XL_2, PixArtBlock, PixArtMS, PixArtMS_XL_2, PixArtMSBlock,  # noqa: F401
                     build_model, install_into_reference, set_grad_checkpoint)
 from .dmd import DMDDistiller, DMDSampler, ddpm_alphas_cumprod, null_caption  # noqa: F401
-from .lora import inject_lora, load_adapter, merge_lora, save_adapter, unmerge_lora  # noqa: F401
+from .lora import (inject_dora, inject_lora, load_adapter, load_dora_adapter, merge_lora, save_adapter,  # noqa: F401
+                   unmerge_lora)
 from .lcm import LCMDistiller, LCMSampler, LCMScheduler  # noqa: F401
 from .sa_sampler import SASolverSampler  # noqa: F401
 from .sampler import DPMS, DPMSolverPP  # noqa: F401

@@ -24,6 +24,12 @@ tail_w=s B)`), so every epilogue sees the sum.  Backward: v = s dY B (skinny GEM
 tail v, A^T), dA = v^T X and dB = s dY^T u (weight-gradient form, M = T), straight into lora_A.grad / lora_B.grad when they
 are bucket views.  Weights that do not require grad get no weight-gradient GEMM and no bias column sum.
 
+DoRA: a projection whose adapter carries a magnitude m runs the column-scaled GEMM (`lib.gemm(col_scale=c)`, c = m / wn from
+`lora.prepare_operands`): y = c (x W^T + s u B^T) + b.  Its backward first runs `lib.dora_bwd` on the gradient g of y (and the
+saved y: the projection's output, its GELU pre-activation or its un-gated branch output): dz = c g in place of g, and
+dm += sum_rows g (y - b) / m straight into lora_magnitude.grad when that is a bucket view.  The dgrad, v and dA / dB passes then
+run unchanged on dz.
+
 Parameters may be fp32 (mixed-precision training, `train.py:369` accelerator mixed_precision) or bf16; the kernels
 always consume bf16 shadows, cached per parameter version, and gradients are produced in fp32 and cast to the
 parameter dtype.  There is no eager fallback: a missing library or a non-sm_100 device raises from `lib`.
@@ -99,9 +105,40 @@ def _lora_ops(mod):
     return mod.__dict__.get("_pxa_lora")
 
 
+def _is_dora(mod) -> bool:
+    op = _lora_ops(mod)
+    return op is not None and op.c is not None
+
+
 def _lora_params(mod):
-    """(lora_A, lora_B) of a projection with an active adapter, else (None, None): extra autograd inputs of its node."""
-    return (mod.lora_A, mod.lora_B) if _lora_ops(mod) is not None else (None, None)
+    """(lora_A, lora_B, lora_magnitude) of a projection with an active adapter (magnitude None without DoRA), else
+    (None, None, None): extra autograd inputs of its node."""
+    if _lora_ops(mod) is None:
+        return (None, None, None)
+    return (mod.lora_A, mod.lora_B, mod.lora_magnitude if _is_dora(mod) else None)
+
+
+def _scale(mod) -> dict:
+    """gemm() arguments of the DoRA column scale of `mod`, if any."""
+    return dict(col_scale=_lora_ops(mod).c) if _is_dora(mod) else {}
+
+
+def _dora_bwd(mod, g, y, need_m: bool, inplace: bool):
+    """(dz, dm) of a DoRA projection for the gradient g of its output y = c z + b: dz = c g (over g when `inplace`) and the
+    magnitude gradient, added into lora_magnitude.grad when the kernel may accumulate there (then dm is None).  Without DoRA:
+    (g, None)."""
+    if not _is_dora(mod):
+        return g, None
+    mag = mod.lora_magnitude
+    m32 = mag.detach() if mag.dtype == torch.float32 else mag.detach().float()
+    acc = _grad_accumulator(mag) if need_m else None
+    dm = acc if acc is not None else torch.zeros(mag.shape, dtype=torch.float32, device=g.device)
+    dz = g if inplace else torch.empty_like(g)
+    lib.dora_bwd(g, y, _shadow(mod, "b"), _lora_ops(mod).c, m32, dz, dm)
+    if acc is not None:
+        _grad_landed(mag)
+        return dz, None
+    return dz, (dm if mag.dtype == torch.float32 else dm.to(mag.dtype)) if need_m else None
 
 
 def _lora_u(x, mod):
@@ -165,22 +202,23 @@ class LinearFn(torch.autograd.Function):
     lora_B) are passed as tensors too so that autograd routes their gradients."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, mod, lora_A=None, lora_B=None):
+    def forward(ctx, x, weight, bias, mod, lora_A=None, lora_B=None, lora_magnitude=None):
         assert x.dtype == torch.bfloat16 and x.dim() == 2
         x = x.contiguous()
         out = torch.empty((x.shape[0], weight.shape[0]), dtype=torch.bfloat16, device=x.device)
         u = _lora_u(x, mod)
-        lib.gemm(x, _shadow(mod, "w"), _shadow(mod, "b"), out, **_tail(u, mod, "b"))
-        ctx.save_for_backward(x, weight, bias, u)
+        lib.gemm(x, _shadow(mod, "w"), _shadow(mod, "b"), out, **_tail(u, mod, "b"), **_scale(mod))
+        ctx.save_for_backward(x, weight, bias, u, out if _is_dora(mod) else None)
         ctx.mod = mod
         return out
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight, bias, u = ctx.saved_tensors
+        x, weight, bias, u, y = ctx.saved_tensors
         n = ctx.needs_input_grad
-        dx, dw, db, dA, dB = _linear_backward(n[:3], x, weight, bias, ctx.mod, dy.contiguous(), u=u, lora_needs=n[4:6])
-        return dx, dw, db, None, dA, dB
+        dz, dm = _dora_bwd(ctx.mod, dy.contiguous(), y, n[6], inplace=False)
+        dx, dw, db, dA, dB = _linear_backward(n[:3], x, weight, bias, ctx.mod, dz, u=u, lora_needs=n[4:6])
+        return dx, dw, db, None, dA, dB, dm
 
 
 def _linear_backward(ctx_needs, x, weight, bias, mod, dy, u=None, v=None, lora_needs=(False, False)):
@@ -304,10 +342,13 @@ def _norms_qk(a) -> bool:
     return not isinstance(a.q_norm, torch.nn.Identity)
 
 
+_PER = 5                                            # BlockFn inputs per projection
+
+
 def _block_params(blk):
-    """The block's parameters as BlockFn inputs: per projection in _TAGS order (weight, bias, lora_A, lora_B) (None: no
-    adapter), then (weight, bias) of q_norm and k_norm (qk_norm) and of sr and norm (conv KV compression) where the block
-    has them.  A plain block has 28."""
+    """The block's parameters as BlockFn inputs: per projection in _TAGS order (weight, bias, lora_A, lora_B,
+    lora_magnitude) (None: no adapter / no DoRA), then (weight, bias) of q_norm and k_norm (qk_norm) and of sr and norm (conv
+    KV compression) where the block has them.  A plain block has 35."""
     a, ca, mlp = blk.attn, blk.cross_attn, blk.mlp
     mods = (a.qkv, a.proj, ca.q_linear, ca.kv_linear, ca.proj, mlp.fc1, mlp.fc2)
     extra = ((a.q_norm, a.k_norm) if _norms_qk(a) else ()) + ((a.sr, a.norm) if a.sr_ratio > 1 and a.sampling == "conv" else ())
@@ -374,7 +415,7 @@ def _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, 
         """The projection `lin` (tag in _TAGS) with its adapter's up-projection as the K-tail; u_<tag> kept in t."""
         if _lora_ops(lin) is not None and "u_" + tag not in t:
             t["u_" + tag] = _lora_u(x, lin)
-        return lib.gemm(x, _shadow(lin, "w"), _shadow(lin, "b"), out, **kw, **_tail(t.get("u_" + tag), lin, "b"))
+        return lib.gemm(x, _shadow(lin, "w"), _shadow(lin, "b"), out, **kw, **_tail(t.get("u_" + tag), lin, "b"), **_scale(lin))
 
     t["xn1"] = lib.ln_modulate(x32, mod[:, 0], mod[:, 1], torch.empty((M, C), **bf), mod_batch_stride=ms, rows_per_batch=N)
     t["qkv"] = gemm("qkv", t["xn1"], a.qkv, torch.empty((M, 3 * C), **bf))
@@ -408,7 +449,10 @@ def _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, 
     else:
         t["ao2"], t["lse2"] = kept["ao2"], kept["lse2"]
     t["x2"] = torch.empty((M, C), **f32)
-    gemm("cproj", t["ao2"], ca.proj, t["x2"], epilogue=lib.EPI_BIAS_RESIDUAL, residual=t["x1"], rows_per_batch=N)
+    if _is_dora(ca.proj):                             # its DoRA backward reads the branch output c z + b
+        t["y2"] = torch.empty((M, C), **bf)
+    gemm("cproj", t["ao2"], ca.proj, t["x2"], epilogue=lib.EPI_BIAS_RESIDUAL, residual=t["x1"], rows_per_batch=N,
+         **(dict(out_aux=t["y2"], aux_is_branch=True) if "y2" in t else {}))
     t["xn2"] = lib.ln_modulate(t["x2"], mod[:, 3], mod[:, 4], torch.empty((M, C), **bf), mod_batch_stride=ms, rows_per_batch=N)
     Hd = mlp.fc1.out_features
     t["h"], t["pre"] = torch.empty((M, Hd), **bf), torch.empty((M, Hd), **bf)
@@ -420,7 +464,7 @@ def _block_forward_kernels(blk, x32, cond, mod, kv_len, kv_off, max_keys, B, N, 
 
 
 _SAVED = ("xn1", "qkv", "ao1", "lse1", "y1", "x1", "xb", "qx", "kv", "ao2", "lse2", "x2", "xn2", "h", "pre", "y3")
-_SAVED_EXTRA = ("qkv_pre", "kc", "vc")              # only blocks with qk_norm / KV compression have them
+_SAVED_EXTRA = ("qkv_pre", "kc", "vc", "y2")        # only blocks with qk_norm / KV compression / a DoRA cross_attn.proj
 _KEPT = ("ao1", "lse1", "ao2", "lse2")
 
 
@@ -464,30 +508,37 @@ class BlockFn(torch.autograd.Function):
         dout = dout.contiguous()
         dm = torch.zeros((6, B, C), **f32)                # d(shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp)
         needs = ctx.needs_input_grad[11:]
-        grads = {}
+        grads, dmag = {}, {}
 
         def lin_bwd(tag, x, lin_mod, dy, need_dx=True, v=None):
             i = _TAGS.index(tag)
-            weight, bias = params[4 * i], params[4 * i + 1]
-            n = needs[4 * i:4 * i + 4]
+            weight, bias = params[_PER * i], params[_PER * i + 1]
+            n = needs[_PER * i:_PER * i + 4]
             dx, *g = _linear_backward((need_dx, n[0], n[1]), x, weight, bias, lin_mod, dy, u=t.get("u_" + tag), v=v,
                                       lora_needs=n[2:])
             grads[tag] = g
             return dx
 
+        def dora(tag, lin_mod, g, y):
+            """DoRA: g (the gradient of the projection's output y) becomes dz = c g in place; the magnitude gradient."""
+            dmag[tag] = _dora_bwd(lin_mod, g, y, needs[_PER * _TAGS.index(tag) + 4], inplace=True)[1]
+
         # (3) x3 = x2 + gate_mlp * (fc2(gelu(fc1(xn2))) + b2)
         dy3 = torch.empty((M, C), **bf)
         lib.gate_residual_bwd(dout, t["y3"], mod[:, 5], dy3, dm[5], gate_batch_stride=ms, rows_per_batch=N)
+        dora("fc2", mlp.fc2, dy3, t["y3"])
         v2 = _lora_v(dy3, mlp.fc2, t.get("u_fc2"))
         lin_bwd("fc2", t["h"], mlp.fc2, dy3, need_dx=False, v=v2)
         dpre = torch.empty_like(t["pre"])
         lib.gemm(dy3, _shadow(mlp.fc2, "t"), None, dpre, epilogue=lib.EPI_MUL_DGELU, residual=t["pre"], **_tail(v2, mlp.fc2, "at"))
+        dora("fc1", mlp.fc1, dpre, t["pre"])
         dxn2 = lin_bwd("fc1", t["xn2"], mlp.fc1, dpre)
         dx2 = torch.empty((M, C), **f32)                  # = dout (the residual path) + the gradient through norm2
         lib.ln_modulate_bwd(t["x2"], dxn2, mod[:, 4], dx2, dm[3], dm[4], mod_batch_stride=ms, rows_per_batch=N, add_in=dout)
         # (2) x2 = x1 + cross_proj(cross_attn(q_linear(bf16(x1)), kv_linear(cond)))
         dy2 = torch.empty((M, C), **bf)
         lib.gate_residual_bwd(dx2, None, None, dy2, None, rows_per_batch=N)
+        dora("cproj", ca.proj, dy2, t.get("y2"))
         dao2 = lin_bwd("cproj", t["ao2"], ca.proj, dy2)
         dq, dkv = torch.empty((M, C), **bf), torch.zeros_like(t["kv"])      # padding key rows get no gradient
         kv4, d4 = t["kv"].view(-1, 2, H, D), dkv.view(-1, 2, H, D)
@@ -495,6 +546,8 @@ class BlockFn(torch.autograd.Function):
                            Nk=max_keys, kv_rows=t["kv"].shape[0], kv_len=kv_len, kv_off=kv_off, q_strides=(C, D),
                            k_strides=(2 * C, D), v_strides=(2 * C, D), dq_strides=(C, D), dk_strides=(2 * C, D),
                            dv_strides=(2 * C, D), scale=ca.head_dim ** -0.5)
+        dora("q", ca.q_linear, dq, t["qx"])
+        dora("kv", ca.kv_linear, dkv, t["kv"])
         dxb = lin_bwd("q", t["xb"], ca.q_linear, dq)
         dcond = lin_bwd("kv", cond, ca.kv_linear, dkv)
         dx1 = torch.empty((M, C), **f32)
@@ -502,6 +555,7 @@ class BlockFn(torch.autograd.Function):
         # (1) x1 = x + gate_msa * (proj(attn(qkv(xn1))) + b)
         dy1 = torch.empty((M, C), **bf)
         lib.gate_residual_bwd(dx1, t["y1"], mod[:, 2], dy1, dm[2], gate_batch_stride=ms, rows_per_batch=N)
+        dora("proj", a.proj, dy1, t["y1"])
         dao1 = lin_bwd("proj", t["ao1"], a.proj, dy1)
         compressed = a.sr_ratio > 1
         dqkv = torch.zeros_like(t["qkv"]) if compressed else torch.empty_like(t["qkv"])  # k / v rows no kept key reads: 0
@@ -527,11 +581,13 @@ class BlockFn(torch.autograd.Function):
                                     rows_per_batch=M, eps=ln.eps)
                 dqkv[:, i * C:(i + 1) * C] = dxs
                 qk_grads += [dsc.view(C), dsh.view(C)]
+        dora("qkv", a.qkv, dqkv, t["qkv_pre"] if _norms_qk(a) else t["qkv"])
         dxn1 = lin_bwd("qkv", t["xn1"], a.qkv, dqkv)
         dx = torch.empty((M, C), **f32)
         lib.ln_modulate_bwd(x32, dxn1, mod[:, 1], dx, dm[0], dm[1], mod_batch_stride=ms, rows_per_batch=N, add_in=dx1)
-        pg = [g for tag in _TAGS for g in grads[tag]]
-        pg += [g.to(p.dtype) if n else None for g, p, n in zip(qk_grads + kv_grads, params[28:], needs[28:])]
+        pg = [g for tag in _TAGS for g in grads[tag] + [dmag[tag]]]
+        np_ = _PER * len(_TAGS)
+        pg += [g.to(p.dtype) if n else None for g, p, n in zip(qk_grads + kv_grads, params[np_:], needs[np_:])]
         return (None, dx, dcond, dm.permute(1, 0, 2), None, None, None, None, None, None, None, *pg)
 
 

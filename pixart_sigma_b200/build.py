@@ -7,7 +7,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpixart_sm100.so")
 SOURCES = ["api.cu", "gemm_sm100.cu", "elementwise_sm100.cu", "attn_sm90.cu", "attn_bwd_sm90.cu", "backward_sm100.cu", "t5_attn_sm90.cu",
-           "optim_sm90.cu", "lcm_sm90.cu", "dmd_sm90.cu", "iddpm_sm90.cu", "vae_out_sm90.cu"]
+           "optim_sm90.cu", "lcm_sm90.cu", "dmd_sm90.cu", "iddpm_sm90.cu", "vae_out_sm90.cu",
+           "dora_sm90.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 

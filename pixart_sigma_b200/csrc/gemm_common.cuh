@@ -39,6 +39,9 @@ struct GemmParams {
   // widths that do not tile (neither a power of two <= 128 nor a multiple of 128): the M index runs over a VIRTUAL image of width
   // conv_Wp = W rounded up to 128 -- pixel columns >= W are TMA zero fill on the way in and are not stored on the way out
   int conv_Wp;
+  // per-output-column scale of the accumulator (kScale, pxa_gemm_dora_bf16): staged in EpiConst::ex1, which the scaled forms
+  // do not otherwise use (they take no aux_scale)
+  const float* col_scale;
 };
 
 inline void fill_ln_params(GemmParams& p, const PxaGemmArgs& a) {
@@ -114,7 +117,7 @@ template <int BN> struct EpiRegs {
   int row_split;
 };
 
-template <int BN, bool kLn = false>
+template <int BN, bool kLn = false, bool kScale = false>
 PXA_DEVICE void load_epi_consts(EpiRegs<BN>& r, const GemmParams& p, int tid, int m0, int n0) {
   const int b0 = m0 / p.rows_per_batch;
   const int last = (m0 + kBM - 1 < p.M ? m0 + kBM - 1 : p.M - 1);
@@ -134,7 +137,8 @@ PXA_DEVICE void load_epi_consts(EpiRegs<BN>& r, const GemmParams& p, int tid, in
       r.v[i][1] = (ok && p.gate != nullptr) ? __ldg(p.gate + (size_t)b0 * p.gate_batch_stride + col) : 1.f;
       r.v[i][2] = (ok && p.gate != nullptr) ? __ldg(p.gate + (size_t)b1 * p.gate_batch_stride + col) : 1.f;
       r.v[i][3] = (ok && p.aux_scale != nullptr) ? __ldg(p.aux_scale + (size_t)b0 * p.aux_scale_batch_stride + col) : 1.f;
-      r.v[i][4] = (ok && p.aux_scale != nullptr) ? __ldg(p.aux_scale + (size_t)b1 * p.aux_scale_batch_stride + col) : 1.f;
+      if constexpr (kScale) r.v[i][4] = ok ? __ldg(p.col_scale + col) : 1.f;
+      else r.v[i][4] = (ok && p.aux_scale != nullptr) ? __ldg(p.aux_scale + (size_t)b1 * p.aux_scale_batch_stride + col) : 1.f;
     }
   }
   r.row_split = (b0 + 1) * p.rows_per_batch - m0;

@@ -20,6 +20,9 @@
 // K-blocks from the tail operands (tail_a [M, tail_k], tail_w [N, tail_k]) into the same ring, and the consumers run the same
 // wgmma loop over them: the epilogue sees A W^T + tail_a tail_w^T.  TMA zero-fills the columns past tail_k.
 //
+// Column scale (kScale, pxa_gemm_dora_bf16): the epilogue multiplies accumulator column n by col_scale[n] before anything
+// else (bias, GELU, gate, residual, aux copies), the DoRA magnitude-over-norm factor of an adapted projection.
+//
 // Algorithmic work: 2*M*N*K FLOP; bytes: M*K*2 (A) + N*K*2 (W) + M*N*out bytes (+ residual read).
 #include "gemm_common.cuh"
 
@@ -50,7 +53,7 @@ PXA_DEVICE int release_kb(int nk) {
 // tmap_out / tmap_res: `out` and the epilogue operand as 3-D tensors (column, x, line) with 32 x 128 x 1 boxes.  x runs over
 // the GEMM rows (one line), except for a convolution over a virtual width, where it runs over the W real pixels of an image
 // line: the stores drop the columns x >= W and the rows >= M.
-template <int BN, int EPI, typename OutT, bool kConv = false, bool kMn = false, bool kTail = false>
+template <int BN, int EPI, typename OutT, bool kConv = false, bool kMn = false, bool kTail = false, bool kScale = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                  const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_res, const GemmParams p,
@@ -64,6 +67,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   constexpr int kSlabs = NW / 32;                  // output slabs per consumer warpgroup
   static_assert(!kMn || NW % 64 == 0, "MN-major W is staged in 64-column atoms");
   static_assert(!kTail || (!kConv && !kMn && !kLn), "the K-tail belongs to the K-major, non-LayerNorm forms");
+  static_assert(!kScale || (!kConv && !kMn && !kLn && EPI != PXA_EPI_MUL_DGELU), "the column scale belongs to the forward forms");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* otile = smem + kStages * Cfg::kStage;                                  // output tile: slab cs at cs * kSlabBytes
@@ -190,7 +194,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     [[maybe_unused]] LnStatRegs sr;
     if ((int)blockIdx.x < num_tiles) {
       const int ft = eff(blockIdx.x);
-      load_epi_consts<BN, kLn>(er, p, tid, tile_m0(ft), tile_n0(ft));
+      load_epi_consts<BN, kLn, kScale>(er, p, tid, tile_m0(ft), tile_n0(ft));
       if constexpr (kLn) if (g == 0) load_ln_stats(sr, p, tile_m0(ft) + tid);
     }
     float acc[2][NW / 2];
@@ -270,7 +274,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
               const int c = 8 * jj + 2 * (lane & 3);                // column in the slab
               const int tc = 32 * cs + c;                           // column in the tile
               const int gcol = n0 + tc;
-              const float a0 = acc[i][4 * (4 * s + jj) + 2 * h], a1 = acc[i][4 * (4 * s + jj) + 2 * h + 1];
+              float a0 = acc[i][4 * (4 * s + jj) + 2 * h], a1 = acc[i][4 * (4 * s + jj) + 2 * h + 1];
+              if constexpr (kScale) {
+                const float2 cs = *reinterpret_cast<const float2*>(cb->ex1 + tc);
+                a0 *= cs.x;
+                a1 *= cs.y;
+              }
               uint8_t* e = slab + slab_offset<OutT>(row, c);
               const bool aux_ok = aux != nullptr && grow < p.M && gcol < p.N;
               const size_t off = (size_t)grow * p.ldo + gcol;
@@ -341,7 +350,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       }
       if (t + (int)gridDim.x < num_tiles) {                          // next tile's loads: in flight during the next main loop
         const int nt_ = eff(t + gridDim.x);
-        load_epi_consts<BN, kLn>(er, p, tid, tile_m0(nt_), tile_n0(nt_));
+        load_epi_consts<BN, kLn, kScale>(er, p, tid, tile_m0(nt_), tile_n0(nt_));
         if constexpr (kLn) if (g == 0) load_ln_stats(sr, p, tile_m0(nt_) + tid);
       }
       // the warpgroup's slabs are written: one thread hands them to the TMA engine
@@ -407,9 +416,9 @@ struct ConvGeom {
   int Wp;          // virtual width of the M index (= W when W tiles; else W rounded up to 128, see GemmParams::conv_Wp)
 };
 
-template <int BN, int EPI, typename OutT, bool kConv = false, bool kMn = false, bool kTail = false>
+template <int BN, int EPI, typename OutT, bool kConv = false, bool kMn = false, bool kTail = false, bool kScale = false>
 static int launch_gemm(const PxaGemmArgs& a, cudaStream_t stream, const ConvGeom* cg = nullptr, int k_splits = 1,
-                       const PxaGemmTail* tl = nullptr) {
+                       const PxaGemmTail* tl = nullptr, const float* col_scale = nullptr) {
   CUtensorMap ta, tw;
   if constexpr (kMn) {
     // A stored [K, M] (row stride lda), W stored [K, N] (row stride ldw): 64 x 64 boxes, M / N the contiguous dimension
@@ -493,7 +502,8 @@ static int launch_gemm(const PxaGemmArgs& a, cudaStream_t stream, const ConvGeom
     p.conv_cin_blocks = cg->Cin / kBK;
   }
   p.conv_Wp = kConv ? cg->Wp : 0;
-  auto kern = gemm_bf16_kernel<BN, EPI, OutT, kConv, kMn, kTail>;
+  p.col_scale = col_scale;
+  auto kern = gemm_bf16_kernel<BN, EPI, OutT, kConv, kMn, kTail, kScale>;
   PXA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   int grid = device_info().sms;
   if (a.max_ctas > 0 && a.max_ctas < grid) grid = a.max_ctas;
@@ -505,22 +515,25 @@ static int launch_gemm(const PxaGemmArgs& a, cudaStream_t stream, const ConvGeom
   return PXA_OK;
 }
 
-template <int BN, bool kTail = false>
-static int dispatch_epi(const PxaGemmArgs& a, cudaStream_t s, const PxaGemmTail* tl = nullptr) {
+template <int BN, bool kTail = false, bool kScale = false>
+static int dispatch_epi(const PxaGemmArgs& a, cudaStream_t s, const PxaGemmTail* tl = nullptr, const float* cs = nullptr) {
   switch (a.epilogue) {
     case PXA_EPI_BIAS:
       if (a.out_dtype != PXA_DTYPE_BF16) return fail(PXA_ERR_ARG, "EPI_BIAS writes bf16 only");
-      return launch_gemm<BN, PXA_EPI_BIAS, __nv_bfloat16, false, false, kTail>(a, s, nullptr, 1, tl);
+      return launch_gemm<BN, PXA_EPI_BIAS, __nv_bfloat16, false, false, kTail, kScale>(a, s, nullptr, 1, tl, cs);
     case PXA_EPI_BIAS_GELU:
       if (a.out_dtype != PXA_DTYPE_BF16) return fail(PXA_ERR_ARG, "EPI_BIAS_GELU writes bf16 only");
-      return launch_gemm<BN, PXA_EPI_BIAS_GELU, __nv_bfloat16, false, false, kTail>(a, s, nullptr, 1, tl);
+      return launch_gemm<BN, PXA_EPI_BIAS_GELU, __nv_bfloat16, false, false, kTail, kScale>(a, s, nullptr, 1, tl, cs);
     case PXA_EPI_BIAS_GELU_AUX:
-      return launch_gemm<BN, PXA_EPI_BIAS_GELU_AUX, __nv_bfloat16, false, false, kTail>(a, s, nullptr, 1, tl);
+      return launch_gemm<BN, PXA_EPI_BIAS_GELU_AUX, __nv_bfloat16, false, false, kTail, kScale>(a, s, nullptr, 1, tl, cs);
     case PXA_EPI_MUL_DGELU:
-      return launch_gemm<BN, PXA_EPI_MUL_DGELU, __nv_bfloat16, false, false, kTail>(a, s, nullptr, 1, tl);
+      if constexpr (kScale) return fail(PXA_ERR_ARG, "the column scale does not take EPI_MUL_DGELU");
+      else return launch_gemm<BN, PXA_EPI_MUL_DGELU, __nv_bfloat16, false, false, kTail>(a, s, nullptr, 1, tl);
     case PXA_EPI_LN_BIAS:
     case PXA_EPI_LN_BIAS_GELU:
-      if constexpr (kTail) {
+      if constexpr (kScale) {
+        return fail(PXA_ERR_ARG, "the column scale does not take the fused LayerNorm epilogues");
+      } else if constexpr (kTail) {
         return fail(PXA_ERR_ARG, "the K-tail does not take the fused LayerNorm epilogues");
       } else {
         if (a.epilogue == PXA_EPI_LN_BIAS) return launch_gemm<BN, PXA_EPI_LN_BIAS, __nv_bfloat16>(a, s);
@@ -529,8 +542,9 @@ static int dispatch_epi(const PxaGemmArgs& a, cudaStream_t s, const PxaGemmTail*
     case PXA_EPI_BIAS_RESIDUAL:
       if (a.residual == nullptr) return fail(PXA_ERR_ARG, "EPI_BIAS_RESIDUAL needs residual");
       if (a.out_dtype == PXA_DTYPE_F32)
-        return launch_gemm<(BN == 256 || kTail) ? 128 : BN, PXA_EPI_BIAS_RESIDUAL, float, false, false, kTail>(a, s, nullptr, 1, tl);
-      return launch_gemm<BN, PXA_EPI_BIAS_RESIDUAL, __nv_bfloat16, false, false, kTail>(a, s, nullptr, 1, tl);
+        return launch_gemm<(BN == 256 || kTail || kScale) ? 128 : BN, PXA_EPI_BIAS_RESIDUAL, float, false, false, kTail, kScale>(
+            a, s, nullptr, 1, tl, cs);
+      return launch_gemm<kScale ? 128 : BN, PXA_EPI_BIAS_RESIDUAL, __nv_bfloat16, false, false, kTail, kScale>(a, s, nullptr, 1, tl, cs);
     default:
       return fail(PXA_ERR_ARG, "unknown epilogue %d", a.epilogue);
   }
@@ -607,7 +621,7 @@ extern "C" int pxa_conv3x3_nhwc_bf16(const PxaConv3x3Args* args, void* stream) {
 }
 
 namespace pxa {
-static int gemm_impl(const PxaGemmArgs* args, const PxaGemmTail* tl, void* stream) {
+static int gemm_impl(const PxaGemmArgs* args, const PxaGemmTail* tl, const float* col_scale, void* stream) {
   if (!args) return fail(PXA_ERR_ARG, "null args");
   const PxaGemmArgs& a = *args;
   if (!a.a || !a.w || !a.out) return fail(PXA_ERR_ARG, "null a / w / out");
@@ -633,6 +647,14 @@ static int gemm_impl(const PxaGemmArgs* args, const PxaGemmTail* tl, void* strea
     if ((tl->lda_tail & 7) || (tl->ldw_tail & 7))
       return fail(PXA_ERR_ALIGN, "lda_tail / ldw_tail must be multiples of 8 (got %d, %d)", tl->lda_tail, tl->ldw_tail);
     if (tl->lda_tail < tl->tail_k || tl->ldw_tail < tl->tail_k) return fail(PXA_ERR_ARG, "lda_tail / ldw_tail < tail_k");
+  }
+  if (col_scale) {
+    if (a.operands_mn_major) return fail(PXA_ERR_ARG, "the column scale does not take operands_mn_major");
+    if (a.epilogue != PXA_EPI_BIAS && a.epilogue != PXA_EPI_BIAS_GELU && a.epilogue != PXA_EPI_BIAS_GELU_AUX &&
+        a.epilogue != PXA_EPI_BIAS_RESIDUAL)
+      return fail(PXA_ERR_ARG, "the column scale takes EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_GELU_AUX and EPI_BIAS_RESIDUAL only");
+    if (a.aux_scale || a.row_stats_out) return fail(PXA_ERR_ARG, "the column scale does not take aux_scale / row_stats_out");
+    if (reinterpret_cast<uintptr_t>(col_scale) & 3) return fail(PXA_ERR_ALIGN, "col_scale must be 4-byte aligned");
   }
   PXA_REQUIRE_SM90();
   int bn = a.block_n;
@@ -678,12 +700,29 @@ static int gemm_impl(const PxaGemmArgs* args, const PxaGemmTail* tl, void* strea
   // the tail instantiations spill at BN 256 and, with fp32 output, at BN 192: they run at 192 and 128 instead
   if (tl && bn == 256) bn = 192;
   if (tl && bn == 192 && a.out_dtype == PXA_DTYPE_F32) bn = 128;
+  // the column-scaled instantiations spill at BN 256 and, with the residual epilogue, at BN 192: they run at 192 and 128
+  if (col_scale && bn == 256) bn = 192;
+  if (col_scale && a.epilogue == PXA_EPI_BIAS_RESIDUAL) bn = 128;
   if (a.row_stats_out && (a.N + bn - 1) / bn > PXA_LN_STAT_PARTS)
     return fail(PXA_ERR_ARG, "row_stats_out: N / block_n = %d column tiles exceed PXA_LN_STAT_PARTS", (a.N + bn - 1) / bn);
+  if (tl && col_scale) {
+    switch (bn) {
+      case 128: return dispatch_epi<128, true, true>(a, s, tl, col_scale);
+      case 192: return dispatch_epi<192, true, true>(a, s, tl, col_scale);
+      default: return fail(PXA_ERR_ARG, "block_n must be 0, 128, 192 or 256 (got %d)", bn);
+    }
+  }
   if (tl) {
     switch (bn) {
       case 128: return dispatch_epi<128, true>(a, s, tl);
       case 192: return dispatch_epi<192, true>(a, s, tl);
+      default: return fail(PXA_ERR_ARG, "block_n must be 0, 128, 192 or 256 (got %d)", bn);
+    }
+  }
+  if (col_scale) {
+    switch (bn) {
+      case 128: return dispatch_epi<128, false, true>(a, s, nullptr, col_scale);
+      case 192: return dispatch_epi<192, false, true>(a, s, nullptr, col_scale);
       default: return fail(PXA_ERR_ARG, "block_n must be 0, 128, 192 or 256 (got %d)", bn);
     }
   }
@@ -696,9 +735,14 @@ static int gemm_impl(const PxaGemmArgs* args, const PxaGemmTail* tl, void* strea
 }
 }  // namespace pxa
 
-extern "C" int pxa_gemm_bf16(const PxaGemmArgs* args, void* stream) { return pxa::gemm_impl(args, nullptr, stream); }
+extern "C" int pxa_gemm_bf16(const PxaGemmArgs* args, void* stream) { return pxa::gemm_impl(args, nullptr, nullptr, stream); }
 
 extern "C" int pxa_gemm_lora_bf16(const PxaGemmArgs* args, const PxaGemmTail* tail, void* stream) {
   if (!tail) return pxa::fail(PXA_ERR_ARG, "null tail");
-  return pxa::gemm_impl(args, tail, stream);
+  return pxa::gemm_impl(args, tail, nullptr, stream);
+}
+
+extern "C" int pxa_gemm_dora_bf16(const PxaGemmArgs* args, const PxaGemmTail* tail, const float* col_scale, void* stream) {
+  if (!col_scale) return pxa::fail(PXA_ERR_ARG, "null col_scale");
+  return pxa::gemm_impl(args, tail, col_scale, stream);
 }

@@ -44,6 +44,23 @@ class GemmTail(C.Structure):
                 ("ldw_tail", C.c_int32)]
 
 
+class DoraNormItem(C.Structure):
+    _fields_ = [("w", C.c_void_p), ("a", C.c_void_p), ("b", C.c_void_p), ("m", C.c_void_p), ("wn", C.c_void_p), ("c", C.c_void_p)]
+
+
+class DoraNormArgs(C.Structure):
+    _fields_ = [("items", C.POINTER(DoraNormItem)), ("n_items", C.c_int32), ("N", C.c_int32), ("K", C.c_int32), ("T", C.c_int32)]
+
+
+DORA_BWD_ROWS = 128
+
+
+class DoraBwdArgs(C.Structure):
+    _fields_ = [("g", C.c_void_p), ("y", C.c_void_p), ("bias", C.c_void_p), ("c", C.c_void_p), ("m", C.c_void_p),
+                ("dz", C.c_void_p), ("dm", C.c_void_p), ("partials", C.c_void_p), ("ldg", C.c_int64), ("ldy", C.c_int64),
+                ("ldz", C.c_int64), ("M", C.c_int32), ("N", C.c_int32)]
+
+
 class LnPrepareArgs(C.Structure):
     _fields_ = [("x", C.c_void_p), ("a_out", C.c_void_p), ("stats_out", C.c_void_p), ("scale", C.c_void_p),
                 ("mod_batch_stride", C.c_int64), ("rows_per_batch", C.c_int32), ("M", C.c_int32), ("C", C.c_int32),
@@ -240,7 +257,7 @@ EXPORTS = ("pxa_transpose_bf16", "pxa_gelu_tanh_bf16", "pxa_gate_residual_fwd", 
            "pxa_t5_attn_d64_bf16", "pxa_sa_solver_step", "pxa_iddpm_step",
            "pxa_grad_clip_flat", "pxa_came_workspace_bytes", "pxa_came_flat",
            "pxa_lcm_step", "pxa_lcm_teacher_target", "pxa_lcm_consistency_loss", "pxa_ema_flat",
-           "pxa_dmd_loss", "pxa_gemm_lora_bf16", "pxa_vae_out_u8")
+           "pxa_dmd_loss", "pxa_gemm_lora_bf16", "pxa_vae_out_u8", "pxa_gemm_dora_bf16", "pxa_dora_norm", "pxa_dora_bwd")
 
 _lib = None
 
@@ -270,12 +287,15 @@ def load() -> C.CDLL:
             fn.argtypes = [C.POINTER(struct), C.c_void_p]
         for name, struct in (("pxa_gate_residual_fwd", GateResidualArgs), ("pxa_gate_residual_bwd", GateResidualArgs),
                              ("pxa_ln_modulate_bwd", LnModBwdArgs), ("pxa_flash_attn_d72_bwd_bf16", AttnBwdArgs),
-                             ("pxa_kv_compress_conv2_ln_bwd", KvCompressBwdArgs)):
+                             ("pxa_kv_compress_conv2_ln_bwd", KvCompressBwdArgs), ("pxa_dora_norm", DoraNormArgs),
+                             ("pxa_dora_bwd", DoraBwdArgs)):
             fn = getattr(lib, name)
             fn.restype = C.c_int
             fn.argtypes = [C.POINTER(struct), C.c_void_p]
         lib.pxa_gemm_lora_bf16.restype = C.c_int
         lib.pxa_gemm_lora_bf16.argtypes = [C.POINTER(GemmArgs), C.POINTER(GemmTail), C.c_void_p]
+        lib.pxa_gemm_dora_bf16.restype = C.c_int
+        lib.pxa_gemm_dora_bf16.argtypes = [C.POINTER(GemmArgs), C.POINTER(GemmTail), C.c_void_p, C.c_void_p]
         lib.pxa_came_workspace_bytes.restype = C.c_int
         lib.pxa_came_workspace_bytes.argtypes = [C.POINTER(CameArgs), C.POINTER(CameParam), C.POINTER(C.c_int64)]
         lib.pxa_layernorm_affine_bf16.restype = C.c_int
@@ -332,7 +352,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: to
          row_stats_out: Optional[torch.Tensor] = None, ln_stats: Optional[torch.Tensor] = None,
          ln_u: Optional[torch.Tensor] = None, ln_v: Optional[torch.Tensor] = None, ln_uv_batch_stride: int = 0,
          ln_dim: int = 0, ln_eps: float = 1e-6, reverse_tiles: bool = False, tail_a: Optional[torch.Tensor] = None,
-         tail_w: Optional[torch.Tensor] = None) -> torch.Tensor:
+         tail_w: Optional[torch.Tensor] = None, col_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out = epilogue(a @ w.T + bias). a (M,K) bf16, w (N,K) bf16 (nn.Linear layout), both K-contiguous.
 
     K-tail (pxa_gemm_lora_bf16): with tail_a (M, T) and tail_w (N, T), bf16 K-contiguous, T a multiple of 8, the epilogue is
@@ -340,7 +360,10 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: to
 
     Fused LayerNorm-modulate (include/pixart_sm100.h, PXA_EPI_LN_BIAS): the fp32 residual epilogue can emit the scaled bf16
     copy `out_aux = out * aux_scale[b]` and the per-row partial sums `row_stats_out` (M, 8, 2); the EPI_LN_* epilogues
-    consume them (`ln_stats`) together with the per-sample vectors `ln_u`, `ln_v` (fp32 views, row b at b * stride)."""
+    consume them (`ln_stats`) together with the per-sample vectors `ln_u`, `ln_v` (fp32 views, row b at b * stride).
+
+    Column scale (pxa_gemm_dora_bf16, a DoRA projection): with col_scale (N,) fp32 the accumulator column n is multiplied by
+    col_scale[n] before the epilogue: out = epilogue(col_scale * (a @ w.T [+ tail]) + bias)."""
     assert a.is_cuda and a.dtype == torch.bfloat16 and w.dtype == torch.bfloat16
     assert a.dim() == 2 and w.dim() == 2 and a.stride(1) == 1 and w.stride(1) == 1 and out.dim() == 2 and out.stride(1) == 1
     M, K = a.shape
@@ -366,16 +389,57 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: to
                     aux_is_branch=int(aux_is_branch), aux_scale=_ptr(aux_scale), aux_scale_batch_stride=aux_scale_batch_stride,
                     row_stats_out=_ptr(row_stats_out), ln_stats=_ptr(ln_stats), ln_u=_ptr(ln_u), ln_v=_ptr(ln_v),
                     ln_uv_batch_stride=ln_uv_batch_stride, ln_dim=ln_dim, ln_eps=ln_eps, reverse_tiles=int(reverse_tiles))
+    if col_scale is not None:
+        assert col_scale.dtype == torch.float32 and col_scale.is_cuda and col_scale.is_contiguous() and col_scale.numel() == N
     if tail_a is None and tail_w is None:
-        _check(load().pxa_gemm_bf16(C.byref(args), _stream()), "pxa_gemm_bf16")
+        if col_scale is not None:
+            _check(load().pxa_gemm_dora_bf16(C.byref(args), None, _ptr(col_scale), _stream()), "pxa_gemm_dora_bf16")
+        else:
+            _check(load().pxa_gemm_bf16(C.byref(args), _stream()), "pxa_gemm_bf16")
         return out
     assert tail_a is not None and tail_w is not None and tail_a.dtype == tail_w.dtype == torch.bfloat16
     assert tail_a.dim() == 2 and tail_w.dim() == 2 and tail_a.stride(1) == 1 and tail_w.stride(1) == 1
     T = tail_a.shape[1]
     assert tail_a.shape[0] == M and tail_w.shape == (N, T)
     tail = GemmTail(tail_a=_ptr(tail_a), tail_w=_ptr(tail_w), tail_k=T, lda_tail=tail_a.stride(0), ldw_tail=tail_w.stride(0))
-    _check(load().pxa_gemm_lora_bf16(C.byref(args), C.byref(tail), _stream()), "pxa_gemm_lora_bf16")
+    if col_scale is not None:
+        _check(load().pxa_gemm_dora_bf16(C.byref(args), C.byref(tail), _ptr(col_scale), _stream()), "pxa_gemm_dora_bf16")
+    else:
+        _check(load().pxa_gemm_lora_bf16(C.byref(args), C.byref(tail), _stream()), "pxa_gemm_lora_bf16")
     return out
+
+
+def dora_norm(items, *, N: int, K: int, T: int) -> None:
+    """pxa_dora_norm over same-shaped projections.  items: (w, a, b, m, wn, c) per projection -- w bf16 [N, K], a bf16 [T, K],
+    b bf16 [N, T] (all contiguous), m fp32 [N] or None, wn / c fp32 [N] outputs or None.  wn = ||w + b a||_2 per row, c = m / wn."""
+    arr = (DoraNormItem * max(len(items), 1))()
+    for i, (w, a, b, m, wn, c) in enumerate(items):
+        assert w.dtype == a.dtype == b.dtype == torch.bfloat16 and w.is_cuda
+        assert w.shape == (N, K) and a.shape == (T, K) and b.shape == (N, T)
+        assert w.is_contiguous() and a.is_contiguous() and b.is_contiguous()
+        for v in (m, wn, c):
+            assert v is None or (v.dtype == torch.float32 and v.is_contiguous() and v.numel() == N)
+        arr[i] = DoraNormItem(w=_ptr(w), a=_ptr(a), b=_ptr(b), m=_ptr(m), wn=_ptr(wn), c=_ptr(c))
+    args = DoraNormArgs(items=arr, n_items=len(items), N=N, K=K, T=T)
+    _check(load().pxa_dora_norm(C.byref(args), _stream()), "pxa_dora_norm")
+
+
+def dora_bwd(g: torch.Tensor, y: torch.Tensor, bias: Optional[torch.Tensor], c: torch.Tensor, m: torch.Tensor,
+             dz: torch.Tensor, dm: torch.Tensor) -> torch.Tensor:
+    """pxa_dora_bwd: dz = bf16(c * g) (dz may be g) and dm += sum_rows g * (y - bias) / m.  g, y, dz bf16 [M, N] (row stride a
+    multiple of 8), bias bf16 [N] or None, c / m / dm fp32 [N].  Returns dz."""
+    M, N = g.shape
+    assert g.dtype == y.dtype == dz.dtype == torch.bfloat16 and y.shape == dz.shape == (M, N)
+    assert g.stride(1) == y.stride(1) == dz.stride(1) == 1
+    for v in (c, m, dm):
+        assert v.dtype == torch.float32 and v.is_contiguous() and v.numel() == N
+    if bias is not None:
+        assert bias.dtype == torch.bfloat16 and bias.is_contiguous() and bias.numel() == N
+    partials = torch.empty(((M + DORA_BWD_ROWS - 1) // DORA_BWD_ROWS, N), dtype=torch.float32, device=g.device)
+    args = DoraBwdArgs(g=_ptr(g), y=_ptr(y), bias=_ptr(bias), c=_ptr(c), m=_ptr(m), dz=_ptr(dz), dm=_ptr(dm),
+                       partials=_ptr(partials), ldg=g.stride(0), ldy=y.stride(0), ldz=dz.stride(0), M=M, N=N)
+    _check(load().pxa_dora_bwd(C.byref(args), _stream()), "pxa_dora_bwd")
+    return dz
 
 
 def ln_prepare(x: torch.Tensor, mult: torch.Tensor, a_out: torch.Tensor, stats_out: torch.Tensor, *, mod_batch_stride: int,
